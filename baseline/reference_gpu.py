@@ -2,8 +2,8 @@
 target ("the reference's own PyTorch/cuDNN build on the same box").
 
 Nothing of esvit_b200 is on this path: the UNMODIFIED `models.swin_transformer.SwinTransformer`,
-`models.vision_transformer.DINOHead` and the `DDINOLoss` class of main_esvit.py (imported from baseline/_ref or
-/root/reference through oracle/reference_import.py's three shims: timm.models.layers, torch._six, AST extraction of the
+`models.vision_transformer.DINOHead` and the `DDINOLoss` class of main_esvit.py (imported from oracle/_ref or
+the reference checkout through oracle/reference_import.py's three shims: timm.models.layers, torch._six, AST extraction of the
 loss classes) are driven through the statement sequence of train_one_epoch (main_esvit.py:507-598):
 
     lr/wd -> autocast{teacher(images[:2]); student(images); loss} -> loss.item() finite check -> zero_grad ->

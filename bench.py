@@ -77,12 +77,14 @@ def parse():
                     help="skip the `gpu_reference` entry (the unmodified reference modules timed on the same GPUs)")
     ap.add_argument("--gpu-ref-steps", type=int, default=10)
     ap.add_argument("--gpu-ref-precisions", default="bf16,fp16")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed to DIR/<name>.npy")
     return ap.parse_args()
 
 
 # ---------------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -131,12 +133,26 @@ class ClockSampler:
                 "samples": len(sm), "reasons": sorted(reasons)}
 
 
-def load_ncu_traffic() -> dict:
-    """{kernel key: {"dram_bytes", "algorithmic_bytes", "ncu_launch", "commit"}} from profiles/ncu_traffic.json."""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-    except Exception:
-        return {}
+DUMP_SAMPLE = 1 << 20  # parameter elements dumped per network (a fixed, seeded sample): 4 MiB of float32 each
+
+
+def dump_outputs(path: str, loss, student, teacher, loss_mod) -> None:
+    """What one training step hands back to its caller: the loss, the updated centers, and a fixed seeded sample of the
+    updated student and teacher parameters (all of them would be ~0.5 GB for the K = 65536 heads).  float32 / float64."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    out = {"loss": np.array([float(loss)], dtype=np.float64)}
+    for name in ("center", "center_grid"):
+        buf = getattr(loss_mod, name, None)
+        if buf is not None:
+            out[name] = buf.detach().float().cpu().numpy()
+    for tag, net in (("student_params_sample", student), ("teacher_params_sample", teacher)):
+        flat = torch.cat([p.detach().reshape(-1).float() for p in net.parameters()])
+        idx = torch.randint(0, flat.numel(), (min(DUMP_SAMPLE, flat.numel()),), generator=torch.Generator().manual_seed(0))
+        out[tag] = flat[idx.to(flat.device)].cpu().numpy()
+        del flat
+    for name, arr in out.items():
+        np.save(os.path.join(path, name + ".npy"), arr)
 
 
 def cuda_parity_loss(arch: str, out_dim: int, n_local: int, batch: int, dev) -> float:
@@ -260,7 +276,7 @@ def run_reference(args):
     kind = "port"
     if device != "cpu":
         from baseline import reference_gpu as RG
-        if RG.available():  # the UNMODIFIED reference modules (baseline/_ref) through train_one_epoch's sequence
+        if RG.available():  # the UNMODIFIED reference modules (oracle/_ref) through train_one_epoch's sequence
             from esvit_b200.engine import SWIN_SPECS
             torch.cuda.set_device(0)
             dev = torch.device("cuda", 0)
@@ -275,7 +291,7 @@ def run_reference(args):
         dt, cores, _ = cpu_reference_steps(args.arch, args.out_dim, args.local_crops, batch, steps, warmup, device)
     val = batch / dt
     sample = f"{steps} steps of batch {batch} ({WORKLOAD}), fp32, oracle port (oracle/step.py), {cores} threads" \
-        if device == "cpu" else (f"{steps} steps of batch {batch}, " + ("unmodified reference modules (baseline/_ref) on cuda"
+        if device == "cpu" else (f"{steps} steps of batch {batch}, " + ("unmodified reference modules (oracle/_ref) on cuda"
                                  if kind == "reference" else "oracle port eager on cuda with bf16 autocast"))
     out = {"impl": "reference", "metric": METRIC, "value": val, "unit": "images/s", "n_gpus": args.gpus,
            "steps": steps, "warmup": warmup, "ms_per_step": dt * 1e3, "higher_is_better": True, "scaling": "weak",
@@ -360,6 +376,8 @@ def main():
     barrier_sync()
     clocks = sampler.stop() if rank == 0 else None
     ms = max_over_ranks(e0.elapsed_time(e1), dev)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, l, student, teacher, loss_mod)
     launches = launches_per_step * K  # esvit_b200 kernels per step (counted in the eager steps) x K
     ms_per_step = ms / K
     value = world * B / (ms_per_step / 1e3)
@@ -414,7 +432,7 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak, peak_src = (peaks["hbm_gbs"], "measured") if "hbm_gbs" in peaks else (6650.0, "fallback")
+    hbm_peak, peak_src = (peaks["hbm_gbs"], "measured") if "hbm_gbs" in peaks else (3350.0, "H100 SXM data sheet")
     roofline, roofline_others = None, []
     if timed:
         def agg(name, bytes_fn, label, extra=None):
@@ -444,24 +462,17 @@ def main():
         # (170 + 98 + 170) rows x K x 2 B per image (SURVEY.md 8d)
         r_ce = agg(ce_bwd_name, lambda t: (2 * rows_s + rows_t) * t["K"] * 2, "dino_ce%s_bwd_kernel (region rows)" % ce_q,
                    extra=lambda t: t["rows"] == rows_s)
-        # tcgen05 fc1 GEMM + bias + GELU: reads A (M*K) and W, writes out and gelu' (2*M*N) in bf16
+        # fc1 GEMM + bias + GELU: reads A (M*K) and W, writes out and gelu' (2*M*N) in bf16
         r_gemm = agg("esvit_gemm_bias_act", lambda t: 2 * (t["M"] * t["K"] + t["N"] * t["K"] + 2 * t["M"] * t["N"]),
-                     "tg::gemm_bias_act_kernel tcgen05 fc1+bias+GELU (all launches of a step)")
+                     "hg::gemm_kernel fc1+bias+GELU (all launches of a step)")
         # same kernel, third epilogue (fc2 dgrad * gelu' + column sums): reads dy (M*K), W2^T, gelu' (M*N), writes d(pre) (M*N)
         r_gemm2 = agg("esvit_gemm_mul_colsum", lambda t: 2 * (t["M"] * t["K"] + t["N"] * t["K"] + 2 * t["M"] * t["N"]),
-                      "tg::gemm_bias_act_kernel tcgen05 fc2-dgrad*gelu'+colsum (all launches of a step)")
-        # dram__bytes_read.sum + dram__bytes_write.sum per launch from `ncu --set full` captures: read from the JSON that
-        # scripts/ncu_summarize.py wrote from the capture (with the commit it was taken at), never pasted in here
-        traffic = load_ncu_traffic()
-        for r, key in ((r_bwd, "window_attn_bwd"), (r_fwd, "window_attn_fwd"), (r_ce, "dino_ce_bwd"),
-                       (r_gemm, "gemm_bias_act"), (r_gemm2, "gemm_mul_colsum")):
-            if r and key in traffic:
-                r["traffic"] = traffic[key]
+                      "hg::gemm_kernel fc2-dgrad*gelu'+colsum (all launches of a step)")
         # second-generation GEMM family (every Linear): bytes = operands read + result written; flops = 2 M N K
         def gemm_bytes(t):
             out_b = 2 * t["M"] * t["N"] * (2 if t.get("pre") else 1)
             return 2 * (t["M"] * t["K"] + t["N"] * t["K"]) + out_b
-        bf_peak = peaks.get("bf16_tflops_sustained", 1400.0)
+        bf_peak = peaks.get("bf16_tflops_sustained", 989.0)  # H100 SXM data sheet, dense
 
         def with_flops(r, name, flops_fn, extra=None):
             if r:
@@ -471,17 +482,17 @@ def main():
                 r["tflops"] = fl / (ms_ / 1e3) / 1e12
                 r["tensor_frac_of_sustained_bf16"] = r["tflops"] / bf_peak
             return r
-        g_fwd = with_flops(agg("esvit_gemm_bf16", gemm_bytes, "tg2::gemm_kernel forward Linear (+bias / +GELU) (all launches of a step)",
+        g_fwd = with_flops(agg("esvit_gemm_bf16", gemm_bytes, "hg::gemm_kernel forward Linear (+bias / +GELU) (all launches of a step)",
                                extra=lambda t: not t["b_mn"]),
                            "esvit_gemm_bf16", lambda t: 2.0 * t["M"] * t["N"] * t["K"], lambda t: not t["b_mn"])
-        g_dgr = with_flops(agg("esvit_gemm_bf16", gemm_bytes, "tg2::gemm_kernel input gradient (MN-major B) (all launches of a step)",
+        g_dgr = with_flops(agg("esvit_gemm_bf16", gemm_bytes, "hg::gemm_kernel input gradient (MN-major B) (all launches of a step)",
                                extra=lambda t: t["b_mn"]),
                            "esvit_gemm_bf16", lambda t: 2.0 * t["M"] * t["N"] * t["K"], lambda t: t["b_mn"])
         g_mul = with_flops(agg("esvit_gemm_mul_colsum2", lambda t: 2 * (t["M"] * t["K"] + t["N"] * t["K"] + 2 * t["M"] * t["N"]),
-                               "tg2::gemm_kernel fc2-dgrad * gelu' + colsum (all launches of a step)"),
+                               "hg::gemm_kernel fc2-dgrad * gelu' + colsum (all launches of a step)"),
                            "esvit_gemm_mul_colsum2", lambda t: 2.0 * t["M"] * t["N"] * t["K"])
         g_wgr = with_flops(agg("esvit_gemm_wgrad", lambda t: 2 * t["T"] * (t["N"] + t["K"]) + 4 * t["N"] * t["K"],
-                               "tg2::gemm_kernel weight gradient (MN-major A and B, split-K) + fold (all launches of a step)"),
+                               "hg::gemm_kernel weight gradient (MN-major A and B, split-K) + fold (all launches of a step)"),
                            "esvit_gemm_wgrad", lambda t: 2.0 * t["T"] * t["N"] * t["K"])
         r_lnf = agg("esvit_add_ln_fwd", lambda t: t["T"] * t["C"] * ((4 if t["has_x"] else 0) + (2 if t["has_delta"] else 0) + 4 + 2),
                     "add_ln_fwd_kernel (all launches of a step)")
@@ -494,9 +505,6 @@ def main():
                     "patch_embed_bwd2_kernel (all launches of a step)")
         # teacher rows once: read bf16 logits, write fp16 probabilities (all launches: cls + region rows)
         r_rsq = agg("esvit_row_softmax_q", lambda t: t["rows"] * t["K"] * 4, "row_softmax_q_kernel (all teacher rows of a step)")
-        for r, key in ((g_fwd, "gemm_bf16"), (g_mul, "gemm_mul_colsum"), (g_wgr, "gemm_wgrad"), (r_lnf, "add_ln_fwd"), (r_lnb, "add_ln_bwd")):
-            if r and key in traffic:
-                r["traffic"] = traffic[key]
         cands = [r for r in (r_bwd, r_fwd, r_ce, r_gemm, r_gemm2, g_fwd, g_dgr, g_mul, g_wgr, r_lnf, r_lnb, r_cef, r_pef, r_peb, r_rsq) if r]
         if cands:
             cands.sort(key=lambda r: -r["ms_per_step"])
@@ -507,10 +515,10 @@ def main():
     step_roofline = None
     gf = GFLOP_PER_IMAGE.get((args.arch, n_local)) if args.out_dim == 65536 else None
     if gf:
-        pk = peaks.get("bf16_tflops_sustained", 1400.0)
+        pk = peaks.get("bf16_tflops_sustained", 989.0)
         ach = gf * value / 1e3 / world  # TFLOP/s per GPU
         step_roofline = {"bound": "tensor", "achieved": ach, "peak": pk, "unit": "TFLOP/s", "frac": ach / pk,
-                         "peak_source": "measured sustained bf16 (MEASURED_PEAKS.json)" if "bf16_tflops_sustained" in peaks else "fallback",
+                         "peak_source": "measured sustained bf16 (MEASURED_PEAKS.json)" if "bf16_tflops_sustained" in peaks else "H100 SXM data sheet, dense bf16",
                          "gflop_per_image_step": gf}
 
     if args.profile and rank == 0:
@@ -559,7 +567,7 @@ def main():
         try:
             from baseline import reference_gpu as RG
             if not RG.available():
-                gpu_reference = {"unavailable": "baseline/_ref missing (run __graft_entry__.build() where /root/reference exists)"}
+                gpu_reference = {"unavailable": "oracle/_ref missing (__graft_entry__.build() installs it where the reference checkout is readable)"}
             else:
                 runs = []
                 for prec in [x for x in args.gpu_ref_precisions.split(",") if x]:
@@ -571,7 +579,7 @@ def main():
                 best = max(runs, key=lambda r: r["value"])
                 gpu_reference = {
                     "what": "UNMODIFIED reference modules (models/swin_transformer.py, models/vision_transformer.py DINOHead, "
-                            "main_esvit.py DDINOLoss; baseline/_ref) driven through train_one_epoch's sequence "
+                            "main_esvit.py DDINOLoss; oracle/_ref) driven through train_one_epoch's sequence "
                             "(main_esvit.py:507-598): autocast, DDP at N>1, per-parameter clip, torch AdamW, EMA loop",
                     "same_config": True, "batch_per_gpu": B, "n_gpus": world, "unit": "images/s",
                     "value": best["value"], "ms_per_step": best["ms_per_step"], "precision": best["precision"], "runs": runs,
@@ -601,7 +609,7 @@ def main():
                           "optimizer": "esvit fused clip+AdamW+EMA" if args.optimizer == "fused" else "torch AdamW fused",
                           "cuda_graph": use_graph,
                           "timed_loop": "loss.item() every step (main_esvit.py:546,596)",
-                          "l2": "per-step working set (>10 GB of activations/logits) >> 126 MB L2; no explicit flush"},
+                          "l2": "per-step working set (>10 GB of activations/logits) >> 50 MB L2; no explicit flush"},
                "gpu_launches": launches, "clocks": clocks, "e2e": e2e, "roofline": roofline, "roofline_others": roofline_others,
                "cpu_baseline": cpu_baseline, "parity_check": parity_check, "gpu_reference": gpu_reference,
                "step_roofline": step_roofline, "peak_mem_gib": own_mem_gib, "loss": last_loss}

@@ -1,4 +1,4 @@
-"""Build libesvit_b200.so (sm_100a) in-tree with nvcc.  No JIT cache: the .so travels with the repo snapshot."""
+"""Build libesvit_b200.so (sm_90a, H100) in-tree with nvcc."""
 from __future__ import annotations
 
 import os
@@ -11,7 +11,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libesvit_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr"]
 
 

@@ -1,4 +1,4 @@
-// Shared device helpers for the esvit_b200 sm_100a kernels.
+// Shared device helpers for the esvit_b200 sm_90a kernels.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -54,7 +54,7 @@ static inline int esvit_num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;  // H100 SXM
   }
   return sms;
 }

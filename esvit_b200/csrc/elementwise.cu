@@ -86,7 +86,7 @@ __global__ void __launch_bounds__(256) gelu_bwd_dbias_kernel(const bf16* __restr
   if (blockIdx.x * 256 + tid < N) atomicAdd(&dbias[blockIdx.x * 256 + tid], a);
 }
 
-// dx = dy * gp (gp = stored local derivative, e.g. gelu'(pre) from the tcgen05 GEMM epilogue); dbias[col] += sum_rows dx.
+// dx = dy * gp (gp = stored local derivative, e.g. gelu'(pre) from the GEMM epilogue); dbias[col] += sum_rows dx.
 // Same tiling as gelu_bwd_dbias_kernel, but pure streaming: 6 B/element, no transcendental math.
 __global__ void __launch_bounds__(256) mul_bwd_dbias_kernel(const bf16* __restrict__ gp, const bf16* __restrict__ dy,
                                                             bf16* __restrict__ dx, float* __restrict__ dbias,

@@ -1,6 +1,6 @@
 // DINOLoss / DDINOLoss kernels: streaming (HBM-bound) passes over the [rows, K] bf16 logits.
 //
-// Reference: /root/reference/main_esvit.py
+// Reference: main_esvit.py
 //   DINOLoss.forward  :620-648     DDINOLoss.forward :683-750     update_center :650-660, :752-770
 //
 // Formulation (DESIGN.md §loss).  With s~ = s / tau_s, t~ = (t - center) / temp and q = softmax(t~):
@@ -327,7 +327,7 @@ __device__ __forceinline__ float fast_ex2(float x) {   // ex2.approx (one SFU in
   asm("ex2.approx.ftz.f32 %0, %1;\n" : "=f"(y) : "f"(x));
   return y;
 }
-constexpr int QT = 512;             // threads of the row-softmax CTA (4 CTAs per SM)
+constexpr int QT = 1024;            // threads of the row-softmax CTA (2 CTAs per SM)
 constexpr float Q_SCALE_LOG2 = 12.f, Q_UNSCALE = 1.f / 4096.f;
 struct __align__(16) half8 { __half2 v[4]; };
 __device__ __forceinline__ void unpack_h8(const half8& h, float* f) {
@@ -335,10 +335,11 @@ __device__ __forceinline__ void unpack_h8(const half8& h, float* f) {
   for (int k = 0; k < 4; k++) { const float2 t = __half22float2(h.v[k]); f[2 * k] = t.x; f[2 * k + 1] = t.y; }
 }
 
-// Two passes over the row: LSE, then q.  The second pass re-reads the 2 K bytes this CTA has just streamed: an L2 hit (the
-// rows in flight on the whole GPU, 592 x 128 KB, fit the 126 MB L2).  A first version kept the row in shared memory: one
+// Two passes over the row: LSE, then q.  The second pass re-reads the 2 K bytes this CTA has just streamed: an L2 hit while
+// the rows in flight on the whole GPU fit the 50 MB L2 - at K = 65536, 132 SMs x 2 CTAs x 128 KB = 33 MB (four 512-thread
+// CTAs per SM would hold 66 MB in flight).  Two 1024-thread CTAs keep the SM's full thread count issuing loads.  A first version kept the row in shared memory: one
 // CTA per SM, its load, reduce and store phases never overlapped, 3x the HBM time.
-__global__ void __launch_bounds__(QT, 4) row_softmax_q_kernel(const bf16* __restrict__ x, const float* __restrict__ center,
+__global__ void __launch_bounds__(QT, 2) row_softmax_q_kernel(const bf16* __restrict__ x, const float* __restrict__ center,
                                                               float inv_temp, float* __restrict__ lse, half8* __restrict__ q, int K) {
   __shared__ float red_m[QT / 32], red_s[QT / 32];
   __shared__ float lse2_sh;

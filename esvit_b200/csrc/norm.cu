@@ -1,7 +1,7 @@
 // Residual-add + LayerNorm, PatchMerging gather + LayerNorm, token mean.  HBM-bound row kernels:
 // one warp per token row, the row lives in registers (float4 per lane), single pass over HBM.
 //
-// Reference semantics (all /root/reference/models/swin_transformer.py):
+// Reference semantics (all models/swin_transformer.py of the reference):
 //   x = shortcut + drop_path(branch); y = norm(x)          :329-331 with :283 of the next block
 //   PatchMerging: 2x2 gather-concat -> LN(4C)               :393-417
 //   final norm + AdaptiveAvgPool1d                          :687-689

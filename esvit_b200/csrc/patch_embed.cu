@@ -217,8 +217,6 @@ __device__ __forceinline__ void pe_gather_tile(const float* __restrict__ img, fl
 template <int EJ>
 __device__ __forceinline__ void pe_conv_tile(const float* As, const float* Ws, const float* bj, int E, int tg, int cg,
                                              float (&acc)[4][EJ]) {
-  // (packed fma.rn.f32x2 over token pairs measured SLOWER here: the shared weight must be duplicated into a register pair
-  // per FMA pair; the weight-gradient loop of the backward, whose operands are natural pairs, does use it)
 #pragma unroll
   for (int i = 0; i < 4; i++)
 #pragma unroll
@@ -315,7 +313,7 @@ __global__ void __launch_bounds__(256) patch_embed_bwd2_kernel(
 #pragma unroll
   for (int j = 0; j < EJ; j++) { bj[j] = bias[cg + 16 * j]; gj[j] = gamma[cg + 16 * j]; }
   const float invE = 1.f / (float)E;
-  // this thread's dW[e = cg+16j][k = tg*3 + kk] (two partial sums each: even / odd token pairs, packed FMAs) and
+  // this thread's dW[e = cg+16j][k = tg*3 + kk] (two partial sums each: even / odd tokens) and
   // per-channel sums
   float2 adw[3][EJ];
   float adb[EJ], adg[EJ], adbe[EJ];
@@ -370,8 +368,10 @@ __global__ void __launch_bounds__(256) patch_embed_bwd2_kernel(
         const float4 d = *reinterpret_cast<const float4*>(Ds + (cg + 16 * j) * PE_LDA + t4 * 4);
 #pragma unroll
         for (int kk = 0; kk < 3; kk++) {
-          adw[kk][j] = __ffma2_rn(make_float2(a[kk].x, a[kk].y), make_float2(d.x, d.y), adw[kk][j]);
-          adw[kk][j] = __ffma2_rn(make_float2(a[kk].z, a[kk].w), make_float2(d.z, d.w), adw[kk][j]);
+          adw[kk][j].x = fmaf(a[kk].x, d.x, adw[kk][j].x);
+          adw[kk][j].y = fmaf(a[kk].y, d.y, adw[kk][j].y);
+          adw[kk][j].x = fmaf(a[kk].z, d.z, adw[kk][j].x);
+          adw[kk][j].y = fmaf(a[kk].w, d.w, adw[kk][j].y);
         }
       }
     }

@@ -1,5 +1,7 @@
 // (Shifted-)window attention core, forward and backward: entry points.  Kernels: window_attn7.cuh (ws = 7, 64-slot
 // windows) and window_attn14.cuh (ws = 14, image-row tiles); persistent CTAs, head = blockIdx.x.
+// A window holds 49 (ws 7) or 196 (ws 14) tokens and head_dim is 32, so a head of a window is a handful of
+// m16n8k16 tiles: the kernels keep S / P / O in warp registers (mma.sync) instead of 64-row warpgroup tiles.
 //
 // Reference: models/swin_transformer.py
 //   WindowAttention.forward :120-152      scores = (q*scale) k^T + rel-pos bias (+ shift mask) -> softmax -> @ v
@@ -20,52 +22,9 @@
 // The backward recomputes P from the saved log-sum-exp (no [B_, nH, N, N] tensor is saved).
 #include <cstdlib>
 
-#include <cuda.h>
 #include "wa_common.cuh"
 #include "window_attn7.cuh"
-#include "window_attn7_tc.cuh"
-#include "window_attn7_tc_bwd.cuh"
 #include "window_attn14.cuh"
-
-namespace wa {
-typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                             const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                             CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeFn get_encode() {
-  static EncodeFn fn = nullptr;
-  if (!fn) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = (EncodeFn)ptr;
-  }
-  return fn;
-}
-// token-major [B, H, W, ch] bf16 tensor seen as (channel, x, y, image); box = 32 channels x 7 x 7 tokens of one image:
-// one head of one window, 49 rows of 64 bytes in shared memory (64B swizzle).  Stores clip what lies outside the image.
-static bool make_window_map(CUtensorMap* map, const void* ptr, int B, int H, int W, int ch, int bx = 7, int by = 7) {
-  EncodeFn enc = get_encode();
-  if (!enc) return false;
-  cuuint64_t dims[4] = {(cuuint64_t)ch, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-  cuuint64_t strides[3] = {(cuuint64_t)ch * 2, (cuuint64_t)W * ch * 2, (cuuint64_t)H * W * ch * 2};
-  cuuint32_t box[4] = {32u, (cuuint32_t)bx, (cuuint32_t)by, 1u};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  return enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-// the nine box shapes of a [B, H, W, ch] output (whole window; the parts of a window that wraps around a shifted image)
-static bool make_out_maps(tc::OutMaps* om, const void* ptr, int B, int H, int W, int ch, int shift) {
-  const int ext[3] = {7, 7 - shift, shift};
-  for (int iy = 0; iy < 3; iy++)
-    for (int ix = 0; ix < 3; ix++) {
-      if (shift == 0 && (ix || iy)) { om->m[iy * 3 + ix] = om->m[0]; continue; }
-      if (!make_window_map(&om->m[iy * 3 + ix], ptr, B, H, W, ch, ext[ix], ext[iy])) return false;
-    }
-  return true;
-}
-}  // namespace wa
 
 namespace wa {
 
@@ -125,27 +84,6 @@ ESVIT_API int esvit_window_attn_fwd(const void* qkv, const void* qkv_bias, const
   if (ws == 7) {
     if (!bias_ws) return ESVIT_ERR_BAD_ARG;
     if (!bias_ready) wa::expand_bias7_kernel<<<nH, 256, 0, st>>>(bias_table, bias_ws, nH);
-    static const int use_tc = [] { const char* e = getenv("ESVIT_ATTN_TC"); return e ? atoi(e) : 2; }();
-    if ((use_tc & 1) && (shift == 0 || shift == 3)) {   // ESVIT_ATTN_TC: bit 0 forward, bit 1 backward
-      // tcgen05 / TMEM forward core: one persistent CTA per SM, head on blockIdx.x, pairs of windows on blockIdx.y
-      const size_t smem_tc = wa::tc::fwd7_tc_smem();
-      cudaError_t e = wa::opt_in_smem(wa::tc::window_attn_fwd7_tc_kernel<true>, smem_tc);
-      if (e == cudaSuccess) e = wa::opt_in_smem(wa::tc::window_attn_fwd7_tc_kernel<false>, smem_tc);
-      if (e != cudaSuccess) return (int)e;
-      const int npairs = (nwin + 1) / 2;
-      int gy = esvit_num_sms() / nH;
-      if (gy < 1) gy = 1;
-      const char* ge = getenv("ESVIT_ATTN_GY");
-      if (ge && atoi(ge) > 0) gy = atoi(ge);
-      if (gy > npairs) gy = npairs;
-      wa::tc::OutMaps tm_out;   // [B, H, W, C] as (channel, x, y, image)
-      if (!wa::make_out_maps(&tm_out, out, B, H, W, C, shift)) return ESVIT_ERR_BAD_ARG;
-      if (shift > 0)
-        wa::tc::window_attn_fwd7_tc_kernel<true><<<dim3(nH, gy), wa::tc::NTHREADS, smem_tc, st>>>(q, qb, bias_ws, (bf16*)out, lse, g, scale, nwin, tm_out);
-      else
-        wa::tc::window_attn_fwd7_tc_kernel<false><<<dim3(nH, gy), wa::tc::NTHREADS, smem_tc, st>>>(q, qb, bias_ws, (bf16*)out, lse, g, scale, nwin, tm_out);
-      ESVIT_LAUNCH_CHECK();
-    }
     const size_t smem = wa::fwd7_smem();
     const int gx = wa::windows_grid(nwin, nH, 16);  // persistent: ~4 waves of 4 resident CTAs per SM
     if (shift > 0)
@@ -182,44 +120,6 @@ ESVIT_API int esvit_window_attn_bwd(const void* qkv, const void* qkv_bias, const
   if (ws == 7) {
     if (!bias_ws) return ESVIT_ERR_BAD_ARG;
     if (!bias_ready) wa::expand_bias7_kernel<<<nH, 256, 0, st>>>(bias_table, bias_ws, nH);
-    static const int use_tc = [] { const char* ev = getenv("ESVIT_ATTN_TC"); return ev ? atoi(ev) : 2; }();   // default: tcgen05
-    if ((use_tc & 2) && (shift == 0 || shift == 3)) {   // (sub-box offsets of the wrapped output parts: 128-byte aligned)
-      // tcgen05 / TMEM backward core: one persistent CTA per SM, head on blockIdx.x, pairs of windows on blockIdx.y
-      const size_t smem_tc = wa::tcb::bwd7_tc_smem();
-      const int npairs = (nwin + 1) / 2;
-      int gy = esvit_num_sms() / nH;
-      if (gy < 1) gy = 1;
-      const char* ge = getenv("ESVIT_ATTN_GY");
-      if (ge && atoi(ge) > 0) gy = atoi(ge);
-      if (gy > npairs) gy = npairs;
-      // [B, H, W, 3C] as (channel, x, y, image); box = one head's 32 channels of one window, or of one wrapped part of it
-      wa::tc::OutMaps tm_dqkv;
-      if (!wa::make_out_maps(&tm_dqkv, dqkv, B, H, W, 3 * C, shift)) return ESVIT_ERR_BAD_ARG;
-      static const int prof = [] { const char* ev = getenv("ESVIT_ATTN_PROF"); return ev ? atoi(ev) : 0; }();
-      static const int ngw = [] { const char* ev = getenv("ESVIT_ATTN_NGW"); return ev ? atoi(ev) : 21; }();  // 21: 2 gather + 1 MMA warp
-      const char* de = getenv("ESVIT_ATTN_DBG");
-      const int dbg = de ? (prof ? atoi(de) : (atoi(de) & 65)) : 0;
-#define WA_TCB_LAUNCH(SH, NG, NM, PR)                                                                                      \
-  do {                                                                                                                     \
-    auto kfn = wa::tcb::window_attn_bwd7_tc_kernel<SH, NG, NM, PR>;                                                        \
-    cudaError_t e2 = wa::opt_in_smem(kfn, smem_tc);                                                                        \
-    if (e2 != cudaSuccess) return (int)e2;                                                                                 \
-    kfn<<<dim3(nH, gy), wa::tcb::nthreads(NG, NM), smem_tc, st>>>(q, qb, bias_ws, (const bf16*)out, (const bf16*)dout,     \
-                                                                  lse, (bf16*)dqkv, dbias_table, dqkv_bias, g, scale,     \
-                                                                  nwin, dbg, tm_dqkv);                                    \
-  } while (0)
-#define WA_TCB_SHIFT(NG, NM, PR) do { if (shift > 0) WA_TCB_LAUNCH(true, NG, NM, PR); else WA_TCB_LAUNCH(false, NG, NM, PR); } while (0)
-      // 20 warps (640 threads x 96 registers): 16 row warps + ngw gather warps + 1 or 2 MMA-issuing warps (ngw 2: one per
-      // quad).  prof: development aid (per-role cycle accounting printed by CTA (0, 0))
-      if (prof) {
-        if (ngw == 2) WA_TCB_SHIFT(2, 2, true); else if (ngw == 21) WA_TCB_SHIFT(2, 1, true); else WA_TCB_SHIFT(3, 1, true);
-      } else {
-        if (ngw == 2) WA_TCB_SHIFT(2, 2, false); else if (ngw == 21) WA_TCB_SHIFT(2, 1, false); else WA_TCB_SHIFT(3, 1, false);
-      }
-#undef WA_TCB_SHIFT
-#undef WA_TCB_LAUNCH
-      ESVIT_LAUNCH_CHECK();
-    }
     const size_t smem = wa::bwd7_smem();
     cudaError_t e = wa::opt_in_smem(wa::window_attn_bwd7_kernel<true>, smem);
     if (e == cudaSuccess) e = wa::opt_in_smem(wa::window_attn_bwd7_kernel<false>, smem);

@@ -156,14 +156,8 @@ __global__ void __launch_bounds__(128, 4) window_attn_fwd7_kernel(
       ldsm_x4(kb, Ks + (nt * 8 + (lane & 7)) * LD + (lane >> 3) * 8);
       mma16816(acc[nt], qa[0], kb[0], kb[1]);
       mma16816(acc[nt], qa[1], kb[2], kb[3]);
-      // the softmax arithmetic runs on column PAIRS (an accumulator fragment holds two adjacent columns of a row) in packed
-      // fp32 (fma.rn.f32x2 ...): half the FMA-pipe instructions, which issue only every second cycle per SMSP
-      {
-        const float2 cc = make_float2(c, c);
-        const float2 a01 = __ffma2_rn(make_float2(acc[nt][0], acc[nt][1]), cc, make_float2(breg[nt][0], breg[nt][1]));
-        const float2 a23 = __ffma2_rn(make_float2(acc[nt][2], acc[nt][3]), cc, make_float2(breg[nt][2], breg[nt][3]));
-        acc[nt][0] = a01.x; acc[nt][1] = a01.y; acc[nt][2] = a23.x; acc[nt][3] = a23.y;
-      }
+#pragma unroll
+      for (int i = 0; i < 4; i++) acc[nt][i] = fmaf(acc[nt][i], c, breg[nt][i]);
       if (SHIFT) {
         const int2 rc = *reinterpret_cast<const int2*>(rid + nt * 8 + (lane & 3) * 2);
         if (ridA != rc.x) acc[nt][0] += -100.f * LOG2E;
@@ -178,20 +172,18 @@ __global__ void __launch_bounds__(128, 4) window_attn_fwd7_kernel(
     m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
     m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 1));
     m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
-    float2 s0p = make_float2(0.f, 0.f), s1p = make_float2(0.f, 0.f);
-    const float2 nm0 = make_float2(-m0, -m0), nm1 = make_float2(-m1, -m1);
+    // two partial sums per row (even / odd column of the fragment pair)
+    float s0x = 0.f, s0y = 0.f, s1x = 0.f, s1y = 0.f;
 #pragma unroll
     for (int nt = 0; nt < C::NT8; nt++) {
-      const float2 x01 = __fadd2_rn(make_float2(acc[nt][0], acc[nt][1]), nm0);
-      const float2 x23 = __fadd2_rn(make_float2(acc[nt][2], acc[nt][3]), nm1);
-      acc[nt][0] = ex2(x01.x);
-      acc[nt][1] = ex2(x01.y);
-      acc[nt][2] = ex2(x23.x);
-      acc[nt][3] = ex2(x23.y);
-      s0p = __fadd2_rn(s0p, make_float2(acc[nt][0], acc[nt][1]));
-      s1p = __fadd2_rn(s1p, make_float2(acc[nt][2], acc[nt][3]));
+      acc[nt][0] = ex2(acc[nt][0] - m0);
+      acc[nt][1] = ex2(acc[nt][1] - m0);
+      acc[nt][2] = ex2(acc[nt][2] - m1);
+      acc[nt][3] = ex2(acc[nt][3] - m1);
+      s0x += acc[nt][0]; s0y += acc[nt][1];
+      s1x += acc[nt][2]; s1y += acc[nt][3];
     }
-    float s0 = s0p.x + s0p.y, s1 = s1p.x + s1p.y;
+    float s0 = s0x + s0y, s1 = s1x + s1y;
     s0 += __shfl_xor_sync(0xffffffffu, s0, 1);
     s0 += __shfl_xor_sync(0xffffffffu, s0, 2);
     s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
@@ -202,14 +194,10 @@ __global__ void __launch_bounds__(128, 4) window_attn_fwd7_kernel(
       if (rA < C::NT) l[rA] = (m0 + lg2(s0)) * LN2;
       if (rB < C::NT) l[rB] = (m1 + lg2(s1)) * LN2;
     }
-    {
-      const float2 i0p = make_float2(i0, i0), i1p = make_float2(i1, i1);
 #pragma unroll
-      for (int nt = 0; nt < C::NT8; nt++) {
-        const float2 p01 = __fmul2_rn(make_float2(acc[nt][0], acc[nt][1]), i0p);
-        const float2 p23 = __fmul2_rn(make_float2(acc[nt][2], acc[nt][3]), i1p);
-        acc[nt][0] = p01.x; acc[nt][1] = p01.y; acc[nt][2] = p23.x; acc[nt][3] = p23.y;
-      }
+    for (int nt = 0; nt < C::NT8; nt++) {
+      acc[nt][0] *= i0; acc[nt][1] *= i0;
+      acc[nt][2] *= i1; acc[nt][3] *= i1;
     }
     float o[4][4];
 #pragma unroll

@@ -1,4 +1,4 @@
-"""nn.Linear layers of the training step on the second-generation tcgen05 GEMM family (csrc/gemm2_tcgen05.cu).
+"""nn.Linear layers of the training step on the wgmma GEMM family (csrc/gemm2_wgmma.cu).
 
 Every GEMM of a Linear - forward, input gradient, weight gradient - is one esvit_b200 kernel:
 

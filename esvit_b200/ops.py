@@ -1,7 +1,7 @@
 """torch.autograd.Function wrappers over the esvit_b200 C ABI (one entry point per kernel).
 
 PyTorch is used here for device memory (caching allocator), the current CUDA stream and autograd bookkeeping;
-all arithmetic of these ops happens in the hand-written sm_100a kernels.  There is no fallback path: every op
+all arithmetic of these ops happens in the hand-written sm_90a kernels.  There is no fallback path: every op
 requires CUDA tensors and the built library.
 """
 from __future__ import annotations
@@ -638,7 +638,7 @@ GEMM_COLSUM_WS_ROWS = 160  # include/esvit_b200.h: esvit_gemm_mul_colsum scratch
 
 
 def gemm_bias_act(a: Tensor, w: Tensor, bias: Optional[Tensor], act: int = 0, want_pre: bool = False):
-    """tcgen05/TMA GEMM: act(a @ w^T + bias) -> bf16 [M, N] (and gelu'(a @ w^T + bias) when act != 0 and want_pre)."""
+    """wgmma/TMA GEMM: act(a @ w^T + bias) -> bf16 [M, N] (and gelu'(a @ w^T + bias) when act != 0 and want_pre)."""
     a, w = _chk(a, BF16, "a"), _chk(w, BF16, "w")
     bias = _chk(bias, F32, "bias")
     K = a.shape[-1]
@@ -652,7 +652,7 @@ def gemm_bias_act(a: Tensor, w: Tensor, bias: Optional[Tensor], act: int = 0, wa
 
 def gemm(a: Tensor, b: Tensor, bias: Optional[Tensor] = None, act: int = 0, want_pre: bool = False, a_mn: bool = False,
          b_mn: bool = False, tile: int = 0):
-    """Second-generation tcgen05 GEMM: act(opA(a) @ opB(b) + bias) -> bf16 [M, N].
+    """wgmma/TMA GEMM: act(opA(a) @ opB(b) + bias) -> bf16 [M, N].
     a: [..., K] (a_mn: [K, M]);  b: [N, K] (b_mn: [K, N] - a Linear weight read as it lies for the input gradient)."""
     a, b = _chk(a, BF16, "a"), _chk(b, BF16, "b")
     bias = _chk(bias, F32, "bias")
@@ -710,7 +710,7 @@ def gemm_wgrad(dy: Tensor, x: Tensor, out: Optional[Tensor] = None, accumulate: 
 
 
 class LinearGeluFn(Function):
-    """gelu(x @ w^T + b) as ONE tcgen05/TMA kernel (esvit_gemm_bias_act): the GEMM epilogue adds the bias, applies the
+    """gelu(x @ w^T + b) as ONE wgmma/TMA kernel (esvit_gemm_bias_act): the GEMM epilogue adds the bias, applies the
     exact GELU and also emits gelu'(pre-activation), so the [T, 4C] hidden tensor is written once and never re-read in
     the forward and the backward's dh = dy * gelu' (+ bias gradient) is a pure streaming kernel; dx / dw are library
     GEMMs."""
@@ -740,7 +740,7 @@ class LinearGeluFn(Function):
 
 
 class MlpFn(Function):
-    """fc2(gelu(fc1(x))) of the Swin MLP (models/swin_transformer.py:31-35) with both GELU passes inside tcgen05 GEMM
+    """fc2(gelu(fc1(x))) of the Swin MLP (models/swin_transformer.py:31-35) with both GELU passes inside wgmma GEMM
     epilogues.  forward: h, gelu' = esvit_gemm_bias_act(x, w1, b1) (one kernel), y = h @ w2^T + b2 (library GEMM).
     backward: d(pre) = (dy @ w2) * gelu' and the fc1 bias gradient come out of ONE kernel (esvit_gemm_mul_colsum, w2t =
     w2^T bf16 [4C, C]); the hidden-sized dh tensor of the unfused chain (GEMM -> multiply kernel) is never written.

@@ -1,6 +1,6 @@
-"""B200-native Swin backbone behind the reference's module names, signatures and state_dict keys.
+"""H100-native Swin backbone behind the reference's module names, signatures and state_dict keys.
 
-Drop-in for /root/reference/models/swin_transformer.py on the pre-training path: same constructor arguments,
+Drop-in for the reference's models/swin_transformer.py on the pre-training path: same constructor arguments,
 same parameter / buffer names (teacher.load_state_dict(student.state_dict()) and checkpoints interchange),
 ``forward(x or list_of_crops)`` returning ``head(cls)`` or the dense 4-tuple exactly as
 ``SwinTransformer.forward`` (models/swin_transformer.py:713-763).
@@ -31,13 +31,13 @@ Tensor = torch.Tensor
 BF16 = torch.bfloat16
 
 
-# fc1 + bias + exact GELU as one tcgen05/TMA GEMM (esvit_gemm_bias_act) instead of library GEMM + GELU kernel
+# fc1 + bias + GELU as one wgmma/TMA GEMM (esvit_gemm_bias_act) instead of library GEMM + GELU kernel
 USE_TCGEN05_FC1 = os.environ.get("ESVIT_TCGEN05_FC1", "1") != "0"
 # run every per-token op (GEMMs, add+LN, MLP) ONCE over the concatenated tokens of all resolution groups of a multi-crop
 # forward instead of once per group; attention / patch merging / pooling launch per group on slices of the same buffers
 # (SwinTransformer._forward_fused_groups).  ESVIT_FUSE_GROUPS=0 restores the reference's per-group loop.
 USE_FUSED_GROUPS = os.environ.get("ESVIT_FUSE_GROUPS", "1") != "0"
-# every Linear (forward, input gradient, weight gradient) on the second-generation tcgen05 GEMM family (esvit_b200.linear)
+# every Linear (forward, input gradient, weight gradient) on the wgmma GEMM family (esvit_b200.linear)
 # instead of library GEMMs; ESVIT_GEMM2=0 restores the library-GEMM path of round 1
 USE_GEMM2 = os.environ.get("ESVIT_GEMM2", "1") != "0"
 

@@ -1,6 +1,6 @@
-/* esvit_b200 C ABI — the drop-in boundary of the B200-native EsViT multi-crop self-distillation step.
+/* esvit_b200 C ABI — the drop-in boundary of the H100-native EsViT multi-crop self-distillation step.
  *
- * Every entry point takes raw DEVICE pointers + sizes + a cudaStream_t (as void*), launches sm_100a kernels on
+ * Every entry point takes raw DEVICE pointers + sizes + a cudaStream_t (as void*), launches sm_90a kernels on
  * that stream and returns an int status: 0 = ok, otherwise a cudaError_t value or ESVIT_ERR_BAD_ARG (1001) for an
  * unsupported shape.  No entry point allocates, frees or synchronises; all buffers (inputs, outputs, workspaces)
  * are owned by the caller (PyTorch's caching allocator on the host side) and must stay alive in stream order.
@@ -68,9 +68,7 @@ int esvit_patch_embed_bwd(const float* img, const float* w, const float* bias, c
  * bias_ready (ws 7): 1 = bias_ws already holds the expansion written by esvit_window_attn_expand_bias for this table
  * (one expansion per table per step instead of one per call), 0 = the call expands it itself.
  * bwd: dqkv fully written; dbias_table fp32 and dqkv_bias fp32 [3C] (complete qkv-bias gradient) ACCUMULATED.
- * ws 7 backward: tcgen05 / TMEM kernel (five tensor-core GEMMs per window pair, dq/dk/dv through 4-D bulk tensor stores:
- * qkv / dqkv / out rows must be 16-byte aligned, which C % 8 == 0 and a 16-byte aligned base guarantee); ws 7 forward
- * and ws 14: mma.sync kernels (ESVIT_ATTN_TC selects, DESIGN.md 4.3). */
+ * Kernels: bf16 mma.sync with S / P / O in warp registers, one persistent CTA loop per head (DESIGN.md 4.3). */
 int esvit_window_attn_expand_bias(const float* bias_table, float* bias_ws, int nH, int ws, void* stream);
 int esvit_window_attn_fwd(const void* qkv, const void* qkv_bias, const float* bias_table, float* bias_ws, int bias_ready,
                           void* out, float* lse, int B, int H, int W, int C, int nH, int ws, int shift, float scale,
@@ -80,28 +78,28 @@ int esvit_window_attn_bwd(const void* qkv, const void* qkv_bias, const float* bi
                           float* dqkv_bias, int B, int H, int W, int C, int nH, int ws, int shift, float scale,
                           void* stream);
 
-/* ---- tcgen05 / TMA GEMM with fused epilogue ------------------------- nn.Linear + Mlp.act, models/swin_transformer.py:31-33
+/* ---- wgmma / TMA GEMM with fused epilogue --------------------------- nn.Linear + Mlp.act, models/swin_transformer.py:31-33
  * out[M,N] (bf16) = act(a[M,K] @ w[N,K]^T + bias[N]); act 0 = identity, 1 = exact GELU (then `pre`, if not NULL, gets
  * gelu'(pre-activation): the backward is dh = dy * pre, see esvit_mul_bwd_dbias).  a, w bf16 row-major (K contiguous), K % 8 == 0, N % 8 == 0, bias fp32 or NULL.
- * TMA-staged 128B-swizzled tiles, tcgen05.mma with the fp32 accumulator in TMEM, persistent over output tiles. */
+ * TMA-staged 128B-swizzled tiles, wgmma with the fp32 accumulator in registers, persistent over output tiles. */
 int esvit_gemm_bias_act(const void* a, const void* w, const float* bias, void* out, void* pre, long long M, int N, int K,
                         int act, void* stream);
 /* out[M,N] (bf16) = (a[M,K] @ w[N,K]^T) * mult[M,N]; colsum[N] (fp32) += column sums of out (caller zero-fills).
  * Same kernel, third epilogue: the fc2 input-gradient GEMM (a = dy, w = W2^T) fused with the GELU backward of fc1
  * (mult = gelu'(pre-activation) from esvit_gemm_bias_act act = 1) and the fc1 bias gradient - what autograd runs as
- * mm + GeluBackward + sum(0) for Mlp.forward, models/swin_transformer.py:31-35.  The multiplier tile is TMA-loaded
- * into the store-staging slot, so it is read once, coalesced, and never touches registers before use.
+ * mm + GeluBackward + sum(0) for Mlp.forward, models/swin_transformer.py:31-35.  The epilogue reads the multiplier
+ * next to the accumulator fragment it scales.
  * ws fp32 [160*N]: caller-owned scratch (per-CTA partial column sums, folded into colsum inside the call). */
 int esvit_gemm_mul_colsum(const void* a, const void* w, const void* mult, void* out, float* colsum, float* ws,
                           long long M, int N, int K, void* stream);
 
-/* ---- second-generation tcgen05 GEMM family (csrc/gemm2_tcgen05.cu): every nn.Linear of the step, forward, input
+/* ---- wgmma GEMM family (csrc/gemm2_wgmma.cu): every nn.Linear of the step, forward, input
  * gradient and weight gradient -------- models/swin_transformer.py:21-37,88-91,125,150,393-420; vision_transformer.py:385-418
- * CTA pairs (tcgen05.mma.cta_group::2, 256 x 256 tiles) or single CTAs; operands K-major or MN-major (the same row-major
- * matrices read "transposed" by TMA + UMMA MN-major descriptors: no transposed copies).
+ * 64 x BN or 128 x BN tiles (1 or 2 consumer warpgroups, BN 128 / 256); operands K-major or MN-major (the same
+ * row-major matrices read "transposed" by TMA + wgmma's transpose bits: no transposed copies).
  * gemm_bf16: out[M,N] (bf16) = act(opA(a) . opB(b) + bias[N]).  a: a_mn = 0 [M,K] | a_mn = 1 [K,M];  b: b_mn = 0 [N,K]
  *   (Linear weight, forward) | b_mn = 1 [K,N] (Linear weight [out = K, in = N], input gradient).  act 0 identity, 1 exact
- *   GELU (pre != NULL also receives gelu'(pre-activation)).  tile: 0 = automatic, else cta_group * 1000 + BN.
+ *   GELU (pre != NULL also receives gelu'(pre-activation)).  tile: 0 = automatic, else warpgroups * 1000 + BN.
  * gemm_mul_colsum2: out = (a . opB(b)) * mult, colsum ACCUMULATED (see esvit_gemm_mul_colsum); ws fp32 [160 * N].
  * gemm_wgrad: dw[N,K] (fp32) (+)= dy[T,N]^T . x[T,K], split over T, deterministic fold of fp32 partial tiles held in ws
  *   (esvit_gemm_wgrad_ws_floats(N, K) fp32 elements).  All of M / N / K / T multiples of 8. */

@@ -8,7 +8,7 @@ legs of ``bench.py`` may use it.
 The oracle is a *functional* plain-PyTorch restatement (fp32, any device, CPU
 by default) of the reference algorithm, operating directly on a reference
 ``state_dict``.  Every function cites the reference file:line it follows
-(paths relative to ``/root/reference``).
+(paths relative to the reference repository).
 
 Pinning: the reference ships no tests, golden vectors or fixtures
 (SURVEY.md §4), so the oracle is pinned against *outputs of the reference

@@ -1,7 +1,7 @@
 """Functional fp32 oracle of DINOLoss / DDINOLoss and the optimiser-side helpers.
 
 TEST INFRASTRUCTURE — see ``oracle/__init__.py``.  Citations are into
-/root/reference/main_esvit.py and /root/reference/utils.py.
+the reference's main_esvit.py and utils.py.
 """
 from __future__ import annotations
 

@@ -1,6 +1,6 @@
-"""Generate tests/golden/*.pt by RUNNING THE UNMODIFIED REFERENCE in the build container.
+"""Generate tests/golden/*.pt by RUNNING THE UNMODIFIED REFERENCE.
 
-TEST INFRASTRUCTURE.  Usage (only where /root/reference exists):
+TEST INFRASTRUCTURE.  Usage (ESVIT_REFERENCE = a reference checkout):
 
     python -m oracle.make_golden            # writes tests/golden/esvit_small.pt and esvit_small_w14.pt
 
@@ -9,7 +9,8 @@ modules (SwinTransformer.forward, DINOHead, DINOLoss/DDINOLoss, utils.clip_gradi
 utils.cancel_gradients_last_layer, utils.get_params_groups, torch.optim.AdamW, the EMA
 loop) on CPU fp32 (the fp32 branch of train_one_epoch, with the undefined `model` at
 :571 read as `student`).  The oracle is asserted against every stored vector while the
-file is written, so a committed fixture is also a record that the oracle matched.
+file is written, so a committed fixture is also a record that the oracle matched.  The fixtures are stored compactly
+(oracle/golden.py): seeded weights and crops are rebuilt on load, large tensors are kept as a seeded sample.
 """
 from __future__ import annotations
 
@@ -19,6 +20,7 @@ import warnings
 
 import torch
 
+from . import golden as GD
 from . import losses as L
 from . import reference_import as R
 from . import step as ST
@@ -32,6 +34,7 @@ SMALL = dict(img_size=112, embed_dim=32, depths=(2, 2, 2), num_heads=(1, 2, 4), 
 SMALL_W14 = dict(img_size=112, embed_dim=32, depths=(2, 2, 2), num_heads=(1, 2, 4), window_size=14)
 HEAD = dict(hidden_dim=128, bottleneck_dim=64)
 K = 384
+WEIGHT_SEED = 0
 HP = dict(lr=5e-4, weight_decay=0.04, clip_grad=3.0, freeze_last_layer=1, momentum_teacher=0.996,
           teacher_temp=0.04, student_temp=0.1, center_momentum=0.9)
 
@@ -46,16 +49,9 @@ def build(dense: bool, seed: int = 0, small=None):
         m.head = ns.DINOHead(m.num_features, K, **HEAD)
         if dense:
             m.head_dense = ns.DINOHead(m.num_features, K, **HEAD)
-    # random (not zero / one) biases, LN affine and bias tables so every term is exercised
-    g = torch.Generator().manual_seed(seed + 2)
-    with torch.no_grad():
-        for n, p in m.named_parameters():
-            if n.endswith(".bias"):
-                p.copy_(torch.randn(p.shape, generator=g) * 0.05)
-            elif p.dim() == 1 and "norm" in n:
-                p.copy_(1 + torch.randn(p.shape, generator=g) * 0.1)
-            elif "relative_position_bias_table" in n:
-                p.copy_(torch.randn(p.shape, generator=g) * 0.5)
+    # seeded weights (random, not zero / one, biases, LN affine and bias tables so every term is exercised) that the
+    # tests rebuild from the seed instead of reading them from the fixture
+    m.load_state_dict(GD.seeded_state_dict(GD.recipe(m.state_dict()), WEIGHT_SEED))
     return ns, spec, m
 
 
@@ -144,26 +140,28 @@ def make(dense: bool, sd_init=None, small=None, compact: bool = False):
     out = dict(
         meta=dict(spec=dict(small, use_dense_prediction=dense), head=HEAD, out_dim=K, batch=B,
                   n_local=n_local if dense else 0, ncrops=ncrops, hp=HP, nsteps=nsteps,
-                  crop_seed=1234, global_size=112, local_size=48,
+                  crop_seed=1234, global_size=112, local_size=48, weight_seed=WEIGHT_SEED,
                   generator="oracle/make_golden.py (reference run on CPU fp32, torch %s)" % torch.__version__),
         losses=[r["loss"] for r in rec], center_after=loss_mod.center.clone(),
         final_student_stats=stats({k: sd_s[k] for k in orc.names}),
         final_teacher_stats=stats({k: sd_t[k] for k in orc.names}),
-        final_teacher_full={k: sd_t[k].clone() for k in FULL_GRADS if k in sd_t},
+        final_teacher_full={k: GD.sample(sd_t[k]) for k in FULL_GRADS if k in sd_t},
         grads_step0_stats=stats(r0["grads"]),
-        grads_step0_full={k: r0["grads"][k] for k in FULL_GRADS if k in r0["grads"]},
+        grads_step0_full={k: GD.sample(r0["grads"][k]) for k in FULL_GRADS if k in r0["grads"]},
     )
+    sd0_stats = stats({k: v for k, v in sd0.items() if v.dtype.is_floating_point})
     if compact:
         so = r0["student_output"]
-        out.update(state_dict={k: v for k, v in sd0.items() if v.dtype.is_floating_point},  # index buffers = closed forms
+        out.update(state_recipe=GD.recipe(sd0), initial_stats=sd0_stats,
                    s_cls_stats=stats(dict(s_cls=so[0].detach(), s_region=so[1].detach(), s_fea=so[2].detach())),
                    s_npatch=list(so[3]))
         return out
     if dense:
-        out.update(state_dict=sd0, crops=crops)
+        out.update(state_recipe=GD.recipe(sd0), initial_stats=sd0_stats)
         so, to = r0["student_output"], r0["teacher_output"]
-        out.update(s_cls=so[0].detach(), s_region=so[1].detach(), s_fea=so[2].detach(), s_npatch=list(so[3]),
-                   t_cls=to[0].detach(), t_region=to[1].detach(), t_fea=to[2].detach(), t_npatch=list(to[3]),
+        # the region features stay whole: the region-match tests take them as inputs
+        out.update(s_cls=GD.sample(so[0]), s_region=GD.sample(so[1]), s_fea=so[2].detach(), s_npatch=list(so[3]),
+                   t_cls=GD.sample(to[0]), t_region=GD.sample(to[1]), t_fea=to[2].detach(), t_npatch=list(to[3]),
                    center_grid_after=loss_mod.center_grid.clone())
         # argmax indices of the first step, recomputed with the reference's own expression (main_esvit.py:735-736)
         Bn, N = B, to[3][0]
@@ -188,9 +186,9 @@ def make(dense: bool, sd_init=None, small=None, compact: bool = False):
 
 if __name__ == "__main__":
     if not R.available():
-        sys.exit("reference tree not found; golden vectors can only be generated in the build container")
+        sys.exit("reference tree not found: set ESVIT_REFERENCE to a checkout of microsoft/esvit")
     dense = make(True)
-    view = make(False, dense["state_dict"])
+    view = make(False, GD.seeded_state_dict(dense["state_recipe"], WEIGHT_SEED))
     os.makedirs(OUT, exist_ok=True)
     path = os.path.join(OUT, "esvit_small.pt")
     torch.save(dict(dense=dense, view=view), path)

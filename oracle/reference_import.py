@@ -1,9 +1,9 @@
-"""Import the UNMODIFIED reference (``/root/reference``) in the build container.
+"""Import the UNMODIFIED reference (a checkout named by ``ESVIT_REFERENCE``, else ``oracle/_ref/``).
 
 TEST / BASELINE INFRASTRUCTURE — ``oracle/make_golden.py``, the (skipped when the
 tree is absent) cross-check tests and ``baseline/reference_gpu.py`` (bench.py's GPU
-reference arm) use this.  The GPU box has no ``/root/reference``: there the tree is the
-verbatim copy under ``baseline/_ref/`` (git-ignored, shipped by gpurun).
+reference arm) use this.  ``oracle/_ref/`` is the git-ignored verbatim copy that
+``oracle/install_reference.py`` makes during ``__graft_entry__.build()``.
 
 Shims (SURVEY.md §8c) — the reference pins timm==0.3.2 and a 2021 torch:
   * ``timm.models.layers`` -> DropPath / to_2tuple / trunc_normal_
@@ -28,11 +28,8 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 def _default_root() -> str:
-    """/root/reference in the build container; on the GPU box the verbatim copy that baseline/install_reference.py put
-    under the (git-ignored, gpurun-shipped) baseline/_ref/."""
-    if os.path.isfile("/root/reference/main_esvit.py"):
-        return "/root/reference"
-    return os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "baseline", "_ref")
+    """the verbatim copy that oracle/install_reference.py put under the (git-ignored) oracle/_ref/"""
+    return os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref")
 
 
 REF_ROOT = os.environ.get("ESVIT_REFERENCE") or _default_root()

@@ -1,7 +1,7 @@
 """Oracle training step: a functional fp32 restatement of train_one_epoch's body.
 
 TEST INFRASTRUCTURE — see ``oracle/__init__.py``.  Mirrors
-/root/reference/main_esvit.py:507-590 (lr/wd set, teacher fwd, student fwd, loss,
+main_esvit.py:507-590 (lr/wd set, teacher fwd, student fwd, loss,
 backward, per-tensor clip, cancel last-layer grads, AdamW, teacher EMA) for one
 process; DDP averaging / center all-reduce are the identity at world_size 1 and are
 modelled by an optional ``all_reduce`` hook for the gloo tests.

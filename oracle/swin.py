@@ -2,7 +2,7 @@
 
 TEST INFRASTRUCTURE — see ``oracle/__init__.py``.  All functions take the
 reference ``state_dict`` (``sd``) and a key prefix, so the weights are
-literally the reference's tensors.  Citations are into /root/reference.
+literally the reference's tensors.  Citations are into the reference repository.
 """
 from __future__ import annotations
 

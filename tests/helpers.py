@@ -2,6 +2,8 @@ import os
 
 import torch
 
+from oracle import golden as _golden
+
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "esvit_small.pt")
 
 
@@ -16,8 +18,13 @@ def assert_close(a, b, tol, name=""):
     assert r < tol, f"{name}: rel l2 error {r:.3e} >= {tol:.1e}"
 
 
-def load_golden():
-    return torch.load(GOLDEN, map_location="cpu", weights_only=False)
+def load_golden(path: str = GOLDEN):
+    """the fixture with its seeded weights and crops rebuilt (oracle/golden.py)"""
+    return _golden.load(path)
+
+
+# (actual, golden) restricted to the elements a fixture stores (large tensors are stored as a seeded sample)
+at_golden = _golden.at_golden
 
 
 # tolerances (documented in DESIGN.md §parity): the CUDA path runs its GEMMs and branch activations in bf16

@@ -43,8 +43,8 @@ def test_no_cpu_fallback_when_library_missing(monkeypatch):
         _lib.load()
 
 
-def test_sass_is_sm100a():
+def test_sass_is_sm90a():
     out = os.popen(f"cuobjdump -lelf {build.LIB} 2>/dev/null").read()
     if not out:
         pytest.skip("cuobjdump unavailable")
-    assert "sm_100a" in out
+    assert "sm_90a" in out

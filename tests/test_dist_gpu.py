@@ -89,7 +89,7 @@ def _worker(rank, world, port, path):
         dist.destroy_process_group()
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_two_rank_nccl_centers_and_gradients_equal_single_process():
     import torch.multiprocessing as mp
     G = load_golden()

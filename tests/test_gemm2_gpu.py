@@ -1,6 +1,6 @@
-"""Second-generation tcgen05 / TMA GEMM family (csrc/gemm2_tcgen05.cu) against fp32 torch on the same bf16 inputs:
+"""wgmma / TMA GEMM family (csrc/gemm2_wgmma.cu) against fp32 torch on the same bf16 inputs:
 forward (K-major operands), input gradient (MN-major B = the Linear weight as it lies), weight gradient (MN-major A and
-B, split-K fp32 partials), every epilogue, every tile shape (1-CTA / CTA-pair x BN 128 / 256), ragged M / N / K."""
+B, split-K fp32 partials), every epilogue, every tile shape (1 / 2 consumer warpgroups x BN 128 / 256), ragged M / N / K."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -9,7 +9,7 @@ from helpers import assert_close
 
 pytestmark = pytest.mark.gpu
 BF16 = torch.bfloat16
-TILES = [1128, 1256, 2128, 2256]  # cta_group * 1000 + BN
+TILES = [1128, 1256, 2128, 2256]  # consumer warpgroups * 1000 + BN
 
 FWD_SHAPES = [(4096, 96, 384), (1000, 192, 768), (300, 384, 1536), (256, 768, 3072), (512, 3072, 768), (777, 64, 96),
               (128, 128, 288), (33, 96, 288), (20000, 96, 96), (640, 256, 4096), (1111, 2048, 256), (260, 96, 16)]
@@ -83,7 +83,7 @@ def test_wgrad_split_k(T, N, K, tile):
 @pytest.mark.parametrize("M,K,N", [(4096, 96, 384), (1000, 192, 768), (300, 384, 1536), (777, 64, 96), (33, 96, 288),
                                    (20000, 96, 384), (40000, 128, 512)])
 def test_mul_colsum(M, K, N, b_mn, tile):
-    """out = (a @ w^T) * mult, colsum += column sums (fc2 dgrad fused with the GELU backward)."""
+    """out = (a @ w^T) * mult, colsum += column sums (fc2 dgrad fused with the GELU backward), bit-reproducible."""
     from esvit_b200 import ops
     torch.manual_seed(M + K + N + 1)
     d = torch.device("cuda:0")
@@ -96,6 +96,9 @@ def test_mul_colsum(M, K, N, b_mn, tile):
     out = ops.gemm_mul_colsum(a, bop, mult, colsum, b_mn=b_mn, tile=tile)
     assert_close(out, ref, 5e-3, "out")
     assert_close(colsum, out.float().sum(0) + 0.5, 2e-4, "colsum of the bf16 output")
+    colsum2 = torch.full((N,), 0.5, device=d)
+    out2 = ops.gemm_mul_colsum(a, bop, mult, colsum2, b_mn=b_mn, tile=tile)
+    assert torch.equal(out2, out) and torch.equal(colsum2, colsum), "column sums must be bit-reproducible"
 
 
 def test_old_entry_points_still_match():

@@ -1,4 +1,4 @@
-"""tcgen05 / TMA GEMM with fused bias (+GELU) epilogue against torch (bf16 inputs, fp32 reference math)."""
+"""wgmma / TMA GEMM with fused bias (+GELU) epilogue against torch (bf16 inputs, fp32 reference math)."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -66,7 +66,7 @@ def test_gemm_speed_vs_library(capsys):
         rows.append((M, K, N, res[0], res[1], 2.0 * M * K * N / res[0] / 1e9))
     with capsys.disabled():
         for r in rows:
-            print("tcgen05 gemm+bias+gelu M=%d K=%d N=%d: %.3f ms (library gemm + gelu kernel %.3f ms) %.0f TFLOP/s" % r)
+            print("wgmma gemm+bias+gelu M=%d K=%d N=%d: %.3f ms (library gemm + gelu kernel %.3f ms) %.0f TFLOP/s" % r)
 
 
 @pytest.mark.parametrize("M,K,N", [(4096, 96, 384), (1000, 192, 768), (300, 384, 1536), (256, 768, 3072),
@@ -153,4 +153,4 @@ def test_gemm_mul_colsum_speed(capsys):
         rows.append((M, C, N, res[0], res[1], (2.0 * M * N * 2 + M * C * 2) / res[0] / 1e6))
     with capsys.disabled():
         for r in rows:
-            print("tcgen05 dgrad*gelu'+colsum M=%d K=%d N=%d: %.3f ms (library gemm + multiply kernel %.3f ms) %.0f GB/s" % r)
+            print("wgmma dgrad*gelu'+colsum M=%d K=%d N=%d: %.3f ms (library gemm + multiply kernel %.3f ms) %.0f GB/s" % r)

@@ -3,7 +3,7 @@ against the CPU oracle: multi-crop forward, DINO/DDINO loss, gradients, and two 
 import pytest
 import torch
 
-from helpers import TOL_BF16_ACT, TOL_BF16_GRAD, assert_close, load_golden, rel
+from helpers import TOL_BF16_ACT, TOL_BF16_GRAD, assert_close, at_golden, load_golden, rel
 
 pytestmark = pytest.mark.gpu
 
@@ -40,12 +40,12 @@ def test_dense_forward_matches_reference_golden():
         t = teacher(crops[:2])
     assert list(s[3]) == D["s_npatch"] and list(t[3]) == D["t_npatch"]
     assert s[0].dtype == torch.bfloat16 and s[2].dtype == torch.float32
-    assert_close(s[0], D["s_cls"], TOL_BF16_ACT, "student cls logits")
-    assert_close(s[1], D["s_region"], TOL_BF16_ACT, "student region logits")
-    assert_close(s[2], D["s_fea"], TOL_BF16_ACT, "student region features")
-    assert_close(t[0], D["t_cls"], TOL_BF16_ACT, "teacher cls logits")
-    assert_close(t[1], D["t_region"], TOL_BF16_ACT, "teacher region logits")
-    assert_close(t[2], D["t_fea"], TOL_BF16_ACT, "teacher region features")
+    assert_close(*at_golden(s[0], D["s_cls"]), TOL_BF16_ACT, "student cls logits")
+    assert_close(*at_golden(s[1], D["s_region"]), TOL_BF16_ACT, "student region logits")
+    assert_close(*at_golden(s[2], D["s_fea"]), TOL_BF16_ACT, "student region features")
+    assert_close(*at_golden(t[0], D["t_cls"]), TOL_BF16_ACT, "teacher cls logits")
+    assert_close(*at_golden(t[1], D["t_region"]), TOL_BF16_ACT, "teacher region logits")
+    assert_close(*at_golden(t[2], D["t_fea"]), TOL_BF16_ACT, "teacher region features")
 
 
 @pytest.mark.parametrize("dense", [True, False])
@@ -63,7 +63,7 @@ def test_loss_and_gradients_match_reference_golden(dense):
     worst = {}
     for k, g_ref in D["grads_step0_full"].items():
         assert named[k].grad is not None, k
-        worst[k] = rel(named[k].grad, g_ref)
+        worst[k] = rel(*at_golden(named[k].grad, g_ref))
     bad = {k: v for k, v in worst.items() if v >= TOL_BF16_GRAD}
     assert not bad, bad
     # every parameter that has a gradient in the reference has one here, with a matching norm
@@ -96,7 +96,7 @@ def test_two_training_steps_match_reference_golden(dense):
         assert_close(loss.center_grid, D["center_grid_after"], 2e-2, "center_grid")
     tn = dict(teacher.named_parameters())
     for k, v in D["final_teacher_full"].items():
-        assert_close(tn[k], v, 1e-3, "teacher " + k)
+        assert_close(*at_golden(tn[k], v), 1e-3, "teacher " + k)
     # last_layer grads were cancelled in epoch 0 -> AdamW skipped weight_v (utils.py:118-123)
     assert torch.equal(dict(student.named_parameters())["head.last_layer.weight_v"].cpu(),
                        G["dense"]["state_dict"]["head.last_layer.weight_v"])

@@ -79,8 +79,7 @@ def test_swin_tiny_k65536_forward_loss_indices_gradients_match_oracle():
     # Gradient gate.  TOL_BF16_GRAD (6e-2 rel-L2) for every parameter, except the three parameter classes whose gradient
     # passes through the WHOLE 12-block bf16 backward and a softmax / LayerNorm at its most sensitive point: for those the
     # reference ALGORITHM itself, run under bf16 autocast, deviates from its own fp32 run by 0.11 - 0.35 rel-L2 on these
-    # very inputs (profiles/r02_reference_algorithm_bf16_autocast_vs_fp32_gradients.txt, scripts/autocast_deviation.py:
-    # stage-0 norm1.bias 0.35, rel-pos bias tables 0.11 - 0.18, patch_embed.proj.weight 0.18; median over all 187
+    # very inputs (stage-0 norm1.bias 0.35, rel-pos bias tables 0.11 - 0.18, patch_embed.proj.weight 0.18; median over all 187
     # tensors 0.03) - the gate for them is 0.12, i.e. tighter than the reference's own mixed-precision noise.
     def tol_for(name: str) -> float:
         if "relative_position_bias_table" in name or name == "patch_embed.proj.weight" or \
