@@ -10,9 +10,12 @@
 //     read "transposed" by TMA boxes of [64 contiguous MN elements x 64 K rows] and wgmma's transpose bits, so
 //     the input-gradient GEMM dX = dY . W reads W[N,K] as it lies and the weight-gradient GEMM dW = dY^T . X reads
 //     dY[T,N] and X[T,K] as they lie: no transposed copies exist anywhere.
-//   * epilogues (template EPI), straight from the accumulator registers: bias -> bf16 | bias + GELU (+ gelu' for the
-//     backward) | accumulator * multiplier + column sums (fc2 dgrad fused with GELU' and the fc1 bias gradient) |
-//     fp32 split-K partials for the weight gradients (deterministic: partial tiles + fold kernel, no atomics).
+//   * epilogues (template EPI): bias -> bf16 | bias + GELU (+ gelu' for the backward) | accumulator * multiplier +
+//     column sums (fc2 dgrad fused with GELU' and the fc1 bias gradient) | fp32 split-K partials for the weight
+//     gradients (deterministic: partial tiles + fold kernel, no atomics).  The bf16 results go out in 64-column chunks:
+//     stmatrix into a 128B-swizzled shared buffer, then one TMA tile store per chunk and consumer warpgroup (full
+//     32-byte sectors, clipped at M / N by the TMA); the multiplier comes in by TMA, issued by the producer during the
+//     mainloop.  The fp32 partials are stored from the registers.
 // Persistent: one CTA per SM, static round-robin over (split, m tile, n tile) work items; the producer runs ahead into
 // the next item's K blocks while the consumers store the previous one.
 #include <cuda.h>
@@ -68,6 +71,36 @@ __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const CUtensorMap
       "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
+// shared -> global tile store; the box is clipped at the tensor's bounds (nothing is written past row M / column N)
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];\n" ::"l"(map), "r"(smem_src),
+               "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;\n" ::: "memory"); }
+// at most N of this thread's committed store groups still read shared memory
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;\n" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;\n" ::: "memory"); }
+// this thread's generic-proxy shared-memory writes become visible to the TMA (async proxy)
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
+__device__ __forceinline__ void named_barrier(int id, int threads) {
+  asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(threads) : "memory");
+}
+// four 8x8 bf16 matrices; lane l addresses row l % 8 of matrix l / 8 and holds row l / 4, columns 2 (l % 4) + {0, 1} of
+// each (the mma accumulator fragment layout)
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};\n" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2),
+               "r"(r3)
+               : "memory");
+}
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];\n"
+               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
+               : "r"(addr)
+               : "memory");
+}
+__device__ __forceinline__ float2 unpack_bf162(uint32_t u) { return __bfloat1622float2(*reinterpret_cast<const bf162*>(&u)); }
 
 // wgmma shared-memory matrix descriptor, 128B swizzle:
 // start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | layout SWIZZLE_128B = 1 [62,64)
@@ -162,33 +195,46 @@ struct Cfg {
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int BAR_BYTES = 256;
-  static constexpr int STAGES_RAW = (SMEM_LIMIT - 1024 /*alignment slack*/ - BAR_BYTES) / STAGE_BYTES;
-  static constexpr int STAGES_MAX = STAGES_RAW > 6 ? 6 : STAGES_RAW;
-  // EPI_MUL: one row of column partials per consumer warp.  Its stages are cut so that the CTA takes no more shared
-  // memory than the other epilogues: a larger shared-memory carve-out shrinks L1, through which the epilogue reads the
-  // multiplier (measured on H100: the partials on top of the full stage count cost 1.5 ms per Swin-T step, one stage
-  // fewer costs nothing measurable).
+  // bf16 epilogue staging: 64-column chunks of the tile, [BM rows][128 B] each, 128B-swizzled like a [64 x 64] TMA box
+  // (consumer warpgroup wg owns the 8 KB at wg * 8192).  EPI_BIAS: two chunk buffers; EPI_GELU: two (out, gelu') pairs;
+  // EPI_MUL: one buffer per chunk of the tile, loaded with the multiplier by TMA and overwritten in place by the result.
+  static constexpr int NCHUNK = BN / 64;
+  static constexpr int CHUNK_BYTES = BM * 128;
+  static constexpr int EP_BYTES = EPI == EPI_BIAS ? 2 * CHUNK_BYTES
+                                : EPI == EPI_GELU ? 4 * CHUNK_BYTES
+                                : EPI == EPI_MUL  ? NCHUNK * CHUNK_BYTES : 0;
+  // EPI_MUL: one row of column partials per consumer warp
   static constexpr int CS_BYTES = EPI == EPI_MUL ? 4 * WG * BN * 4 : 0;
-  static constexpr int STAGES = (STAGES_MAX * STAGE_BYTES - CS_BYTES) / STAGE_BYTES;
-  static constexpr int SMEM = 1024 + STAGES * STAGE_BYTES + CS_BYTES + BAR_BYTES;
+  static constexpr int STAGES_RAW = (SMEM_LIMIT - 1024 /*alignment slack*/ - BAR_BYTES - EP_BYTES - CS_BYTES) / STAGE_BYTES;
+  static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
+  static constexpr int SMEM = 1024 + STAGES * STAGE_BYTES + EP_BYTES + CS_BYTES + BAR_BYTES;
   static constexpr int NTHREADS = 128 * (WG + 1);
-  static_assert(STAGES >= 2, "pipeline needs at least two stages");
+  static_assert(STAGES >= (WG == 2 && BN == 256 ? 3 : 4), "operand ring too shallow");
+  static_assert(SMEM <= SMEM_LIMIT, "shared memory budget");
+  static_assert((2 * STAGES + 2 + 2 * NCHUNK) * 8 <= BAR_BYTES, "mbarrier area");
 };
 
+// map_o: out, map_x: gelu' out (EPI_GELU) or the multiplier in (EPI_MUL); both [64 columns x 64 rows] boxes, 128B swizzle
 template <int WG, int BN, int EPI, int AMN, int BMN>
 __global__ void __launch_bounds__(128 * (WG + 1), 1) gemm_kernel(const __grid_constant__ CUtensorMap map_a,
                                                                  const __grid_constant__ CUtensorMap map_b,
+                                                                 const __grid_constant__ CUtensorMap map_o,
+                                                                 const __grid_constant__ CUtensorMap map_x,
                                                                  const Params p) {
   using C = Cfg<WG, BN, EPI>;
-  constexpr int STAGES = C::STAGES, BM = C::BM;
+  constexpr int STAGES = C::STAGES, BM = C::BM, NCHUNK = C::NCHUNK;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // [STAGES][A | B], every tile 1024-byte aligned in the SHARED address space (swizzle-128B)
+  // [STAGES][A | B] | epilogue chunks | column partials | mbarriers; every tile and chunk 1024-byte aligned in the SHARED
+  // address space (swizzle-128B)
   uint8_t* tiles = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  float* cs_part = reinterpret_cast<float*>(tiles + STAGES * C::STAGE_BYTES);   // [4 WG][BN]
-  uint64_t* full = reinterpret_cast<uint64_t*>(tiles + STAGES * C::STAGE_BYTES + C::CS_BYTES);
+  uint8_t* ep = tiles + STAGES * C::STAGE_BYTES;
+  float* cs_part = reinterpret_cast<float*>(ep + C::EP_BYTES);   // [4 WG][BN]
+  uint64_t* full = reinterpret_cast<uint64_t*>(ep + C::EP_BYTES + C::CS_BYTES);
   uint64_t* empty = full + STAGES;
   uint64_t* cs_full = empty + STAGES;     // EPI_MUL: every consumer warp has written its partials of a tile
   uint64_t* cs_empty = cs_full + 1;       // ... and the fold threads have consumed them
+  uint64_t* mul_full = cs_empty + 1;      // EPI_MUL, per chunk: the multiplier has landed
+  uint64_t* mul_empty = mul_full + NCHUNK;  // ... and the TMA store of the result has read it back out
 
   const int wg = threadIdx.x >> 7;
   const int m_tiles = (p.M + BM - 1) / BM, n_tiles = (p.N + BN - 1) / BN;
@@ -201,6 +247,8 @@ __global__ void __launch_bounds__(128 * (WG + 1), 1) gemm_kernel(const __grid_co
     for (int i = 0; i < STAGES; i++) { mbar_init(&full[i], 1); mbar_init(&empty[i], 128 * WG); }
     mbar_init(cs_full, 4 * WG);
     mbar_init(cs_empty, FOLD_THREADS);
+    if constexpr (EPI == EPI_MUL)
+      for (int i = 0; i < NCHUNK; i++) { mbar_init(&mul_full[i], 1); mbar_init(&mul_empty[i], WG); }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
   __syncthreads();
@@ -211,11 +259,23 @@ __global__ void __launch_bounds__(128 * (WG + 1), 1) gemm_kernel(const __grid_co
     if (threadIdx.x == 128 * WG) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+      int local = 0;
+      if constexpr (EPI == EPI_MUL) asm volatile("prefetch.tensormap [%0];\n" ::"l"(&map_x) : "memory");
+      for (int item = blockIdx.x; item < num_items; item += gridDim.x, local++) {
         const int tile = item % tiles_mn, split = item / tiles_mn;
         const int m0 = (tile / n_tiles) * BM, n0 = (tile % n_tiles) * BN;
         const int kb0 = split * p.kb_per_split;
         int kb1 = kb0 + p.kb_per_split; kb1 = kb1 < k_blocks ? kb1 : k_blocks;
+        // EPI_MUL: multiplier chunk j of this tile, issued after K block kb0 + j so that it lands during the mainloop
+        // while the first operand stages go out ahead of it; its buffer is free once the previous tile's result chunk j
+        // has been stored
+        auto load_mul = [&](int j) {
+          mbar_wait(&mul_empty[j], (local & 1) ^ 1);
+          const uint32_t dst = smem_u32(ep + j * C::CHUNK_BYTES);
+          mbar_expect_tx(&mul_full[j], C::CHUNK_BYTES);
+#pragma unroll
+          for (int h = 0; h < WG; h++) tma_load_2d(dst + h * 8192, &map_x, &mul_full[j], n0 + 64 * j, m0 + 64 * h);
+        };
         for (int kb = kb0; kb < kb1; kb++) {
           mbar_wait(&empty[stage], phase ^ 1);
           const uint32_t sa = smem_u32(tiles + stage * C::STAGE_BYTES), sb = sa + C::A_BYTES;
@@ -235,7 +295,10 @@ __global__ void __launch_bounds__(128 * (WG + 1), 1) gemm_kernel(const __grid_co
               tma_load_2d(sb + j * 8192, &map_b, &full[stage], n0 + j * 64, kb * BK);    // box [64 N][64 K rows]
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          if constexpr (EPI == EPI_MUL) if (kb - kb0 < NCHUNK) load_mul(kb - kb0);
         }
+        if constexpr (EPI == EPI_MUL)
+          for (int j = kb1 - kb0; j < NCHUNK; j++) load_mul(j);
       }
     } else if (EPI == EPI_MUL && threadIdx.x >= 128 * WG + 32 && threadIdx.x < 128 * WG + 32 + FOLD_THREADS) {
       // EPI_MUL column sums: fixed-order fold of the consumer warps' partials of each tile into this CTA's private
@@ -292,53 +355,123 @@ __global__ void __launch_bounds__(128 * (WG + 1), 1) gemm_kernel(const __grid_co
       wgmma_wait<0>();
       if (prev >= 0) mbar_arrive(&empty[prev]);
 
-      // ---- epilogue from registers ----
-      if constexpr (EPI == EPI_MUL) mbar_wait(cs_empty, (local & 1) ^ 1);   // the previous tile's partials are folded
+      if constexpr (EPI == EPI_F32) {
+        // ---- fp32 split-K partials straight from the registers ----
 #pragma unroll
-      for (int i = 0; i < BN / 8; i++) {
-        float cs0 = 0.f, cs1 = 0.f;
-        const int col = n0 + i * 8 + frag_col;
-        if (col >= p.N) continue;  // N % 8 == 0: col + 1 < N as well, and the test is uniform over the warp
-        float b0 = 0.f, b1 = 0.f;
-        if constexpr (EPI == EPI_BIAS || EPI == EPI_GELU) {
-          if (p.bias) { const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + col)); b0 = bb.x; b1 = bb.y; }
+        for (int i = 0; i < BN / 8; i++) {
+          const int col = n0 + i * 8 + frag_col;
+          if (col >= p.N) continue;  // N % 8 == 0: col + 1 < N as well, and the test is uniform over the warp
+#pragma unroll
+          for (int h = 0; h < 2; h++) {
+            const int row = m0 + frag_row + 8 * h;
+            if (row >= p.M) continue;
+            const long long off = (long long)row * p.N + col;
+            *reinterpret_cast<float2*>(p.part + (long long)split * p.M * p.N + off) =
+                make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+          }
+        }
+        continue;
+      }
+
+      // ---- bf16 epilogue: 64-column chunks through swizzled shared memory, one TMA tile store per chunk and warpgroup.
+      // Rows >= M and columns >= N of a box are clipped by the TMA, so there is no bounds test on the stores; the
+      // operands' out-of-bounds rows / columns were zero-filled, so those accumulators (and multipliers) are 0.
+      // ldmatrix / stmatrix lane address: row (lane & 15) of the warp's 16, 16-byte column block (lane >> 4) of a pair;
+      // the 128B swizzle puts 16-byte block c of row r at block c ^ (r & 7): the 8 rows of a matrix hit distinct banks.
+      if constexpr (EPI == EPI_MUL) mbar_wait(cs_empty, (local & 1) ^ 1);   // the previous tile's partials are folded
+      const uint32_t lrow = (uint32_t)(warp * 16 + (lane & 15)) * 128u, lsw = lane & 7, lblk = lane >> 4;
+      const bool leader = t == 0;   // issues this warpgroup's stores and waits for them
+#pragma unroll
+      for (int c = 0; c < NCHUNK; c++) {
+        uint32_t buf;   // this warpgroup's [64 rows][128 B] of the chunk buffer
+        if constexpr (EPI == EPI_MUL) {
+          buf = smem_u32(ep + c * C::CHUNK_BYTES) + wg * 8192;
+          mbar_wait(&mul_full[c], local & 1);
+        } else {
+          buf = smem_u32(ep + (c & 1) * (EPI == EPI_GELU ? 2 : 1) * C::CHUNK_BYTES) + wg * 8192;
         }
 #pragma unroll
-        for (int h = 0; h < 2; h++) {
-          const int row = m0 + frag_row + 8 * h;
-          if (row >= p.M) continue;
-          float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
-          const long long off = (long long)row * p.N + col;
-          if constexpr (EPI == EPI_F32) {
-            *reinterpret_cast<float2*>(p.part + (long long)split * p.M * p.N + off) = make_float2(v0, v1);
-          } else if constexpr (EPI == EPI_MUL) {
-            const float2 m = __bfloat1622float2(*reinterpret_cast<const bf162*>(p.aux + off));
-            const bf162 o = __floats2bfloat162_rn(v0 * m.x, v1 * m.y);
-            *reinterpret_cast<bf162*>(p.out + off) = o;
-            const float2 of = __bfloat1622float2(o);   // column sums of the STORED (bf16) values
-            cs0 += of.x; cs1 += of.y;
-          } else if constexpr (EPI == EPI_GELU) {
-            v0 += b0; v1 += b1;
-            if (p.aux) {
-              float d0, d1;
-              const float y0 = gelu_fwd_grad(v0, d0), y1 = gelu_fwd_grad(v1, d1);
-              *reinterpret_cast<bf162*>(p.out + off) = __floats2bfloat162_rn(y0, y1);
-              *reinterpret_cast<bf162*>(p.aux + off) = __floats2bfloat162_rn(d0, d1);
-            } else {
-              *reinterpret_cast<bf162*>(p.out + off) = __floats2bfloat162_rn(gelu_fwd(v0), gelu_fwd(v1));
+        for (int jj = 0; jj < 8; jj += 2) {
+          const int i = c * 8 + jj;   // 8-column blocks i, i + 1 of the tile
+          const uint32_t addr = buf + lrow + (((jj + lblk) ^ lsw) << 4);
+          const float* a0 = acc + 4 * i;
+          if constexpr (EPI == EPI_MUL) {
+            uint32_t m[4];
+            ldmatrix_x4(addr, m[0], m[1], m[2], m[3]);
+            uint32_t o[4];
+            float cs[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
+#pragma unroll
+            for (int q = 0; q < 4; q++) {   // matrix q: column block i + q / 2, rows + 8 (q % 2)
+              const float2 mf = unpack_bf162(m[q]);
+              o[q] = pack_bf162(a0[2 * q] * mf.x, a0[2 * q + 1] * mf.y);
+              const float2 of = unpack_bf162(o[q]);   // column sums of the STORED (bf16) values
+              cs[q >> 1][0] += of.x; cs[q >> 1][1] += of.y;
+            }
+            stmatrix_x4(addr, o[0], o[1], o[2], o[3]);
+            // reduce over the 8 row groups of the warp (lanes with equal lane % 4) into this warp's row of partials
+#pragma unroll
+            for (int s = 0; s < 2; s++) {
+              float cs0 = cs[s][0], cs1 = cs[s][1];
+#pragma unroll
+              for (int o2 = 4; o2 < 32; o2 <<= 1) {
+                cs0 += __shfl_xor_sync(0xffffffffu, cs0, o2);
+                cs1 += __shfl_xor_sync(0xffffffffu, cs1, o2);
+              }
+              if (lane < 4)
+                *reinterpret_cast<float2*>(cs_part + (wg * 4 + warp) * BN + (i + s) * 8 + frag_col) = make_float2(cs0, cs1);
             }
           } else {
-            *reinterpret_cast<bf162*>(p.out + off) = __floats2bfloat162_rn(v0 + b0, v1 + b1);
+            float b[4] = {0.f, 0.f, 0.f, 0.f};
+            if (p.bias) {
+#pragma unroll
+              for (int s = 0; s < 2; s++) {
+                const int col = n0 + (i + s) * 8 + frag_col;
+                if (col < p.N) {   // N % 8 == 0: col + 1 < N as well
+                  const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+                  b[2 * s] = bb.x; b[2 * s + 1] = bb.y;
+                }
+              }
+            }
+            uint32_t o[4], d[4];
+#pragma unroll
+            for (int q = 0; q < 4; q++) {
+              const float v0 = a0[2 * q] + b[2 * (q >> 1)], v1 = a0[2 * q + 1] + b[2 * (q >> 1) + 1];
+              if constexpr (EPI == EPI_GELU) {
+                if (p.aux) {
+                  float d0, d1;
+                  const float y0 = gelu_fwd_grad(v0, d0), y1 = gelu_fwd_grad(v1, d1);
+                  o[q] = pack_bf162(y0, y1);
+                  d[q] = pack_bf162(d0, d1);
+                } else {
+                  o[q] = pack_bf162(gelu_fwd(v0), gelu_fwd(v1));
+                }
+              } else {
+                o[q] = pack_bf162(v0, v1);
+              }
+            }
+            stmatrix_x4(addr, o[0], o[1], o[2], o[3]);
+            if constexpr (EPI == EPI_GELU)
+              if (p.aux) stmatrix_x4(addr + C::CHUNK_BYTES, d[0], d[1], d[2], d[3]);
           }
         }
-        if constexpr (EPI == EPI_MUL) {
-          // reduce over the 8 row groups of the warp (lanes with equal lane % 4) into this warp's row of partials
-#pragma unroll
-          for (int o = 4; o < 32; o <<= 1) {
-            cs0 += __shfl_xor_sync(0xffffffffu, cs0, o);
-            cs1 += __shfl_xor_sync(0xffffffffu, cs1, o);
+        fence_proxy_async();
+        // EPI_BIAS / EPI_GELU: the next chunk reuses the buffer of the previous one, whose store must have read it out
+        if constexpr (EPI != EPI_MUL)
+          if (leader) bulk_wait_read<0>();
+        named_barrier(1 + wg, 128);
+        if (leader) {
+          const int gc = n0 + 64 * c, gr = m0 + 64 * wg;
+          if (gc < p.N && gr < p.M) {
+            tma_store_2d(&map_o, buf, gc, gr);
+            if constexpr (EPI == EPI_GELU)
+              if (p.aux) tma_store_2d(&map_x, buf + C::CHUNK_BYTES, gc, gr);
           }
-          if (lane < 4) *reinterpret_cast<float2*>(cs_part + (wg * 4 + warp) * BN + i * 8 + frag_col) = make_float2(cs0, cs1);
+          bulk_commit();
+          if constexpr (EPI == EPI_MUL) {
+            // chunk c - 1's buffer has been stored: the producer may load the next tile's multiplier into it
+            if (c > 0) { bulk_wait_read<1>(); mbar_arrive(&mul_empty[c - 1]); }
+            if (c == NCHUNK - 1) { bulk_wait_read<0>(); mbar_arrive(&mul_empty[c]); }
+          }
         }
       }
       if constexpr (EPI == EPI_MUL) {
@@ -346,6 +479,8 @@ __global__ void __launch_bounds__(128 * (WG + 1), 1) gemm_kernel(const __grid_co
         if (lane == 0) mbar_arrive(cs_full);
       }
     }
+    if constexpr (EPI != EPI_F32)
+      if (t == 0) bulk_wait_all();   // the CTA's last stores have completed before it exits
   }
 }
 
@@ -418,6 +553,15 @@ static int launch_cfg(const Call& c, void* stream, int* rows_out) {
   if (!(AMN ? make_map(&ma, c.a, p.K, p.M, 64) : make_map(&ma, c.a, p.M, p.K, C::BM))) return ESVIT_ERR_BAD_ARG;
   // B: K-major [N,K] box [64 K][BN rows] | MN-major [K,N] box [64 N][64 K rows]
   if (!(BMN ? make_map(&mb, c.b, p.K, p.N, 64) : make_map(&mb, c.b, p.N, p.K, BN))) return ESVIT_ERR_BAD_ARG;
+  // bf16 epilogues: out (and gelu' / the multiplier) [M,N] as [64 columns x 64 rows] boxes; the TMA needs 16-byte aligned
+  // base addresses (the row pitch N * 2 B is a multiple of 16 because N % 8 == 0)
+  CUtensorMap mo = {}, mx = {};
+  if (EPI != EPI_F32) {
+    auto aligned = [](const void* q) { return ((uintptr_t)q & 15u) == 0; };
+    if (!p.out || !aligned(p.out) || (p.aux && !aligned(p.aux))) return ESVIT_ERR_BAD_ARG;
+    if (!make_map(&mo, p.out, p.M, p.N, 64)) return ESVIT_ERR_BAD_ARG;
+    if (p.aux && !make_map(&mx, p.aux, p.M, p.N, 64)) return ESVIT_ERR_BAD_ARG;
+  }
   auto kernel = gemm_kernel<WG, BN, EPI, AMN, BMN>;
   static bool attr_set = false;
   if (!attr_set) {
@@ -435,7 +579,7 @@ static int launch_cfg(const Call& c, void* stream, int* rows_out) {
     if (e != cudaSuccess) return (int)e;
   }
   if (rows_out) *rows_out = grid;
-  kernel<<<grid, C::NTHREADS, C::SMEM, (cudaStream_t)stream>>>(ma, mb, p);
+  kernel<<<grid, C::NTHREADS, C::SMEM, (cudaStream_t)stream>>>(ma, mb, mo, mx, p);
   return (int)cudaGetLastError();
 }
 
