@@ -61,6 +61,9 @@ SIGNATURES = {
     "esvit_clip_multi": [P, P, I, F, P, P, P],
     "esvit_grad_sumsq_multi": [P, P, I, P, P],
     "esvit_adamw_ema_multi": [P, P, P, P, P, P, P, P, I, P, P, P, P],
+    "esvit_knn_prep": [P, P, P, P, L, L, I, P],
+    "esvit_knn_select": [P, L, P, P, P, P, P, I, I, I, I, I, P, P, P, P, P, P],
+    "esvit_knn_vote": [P, P, P, P, L, I, F, I, P, P],
 }
 
 _lib = None

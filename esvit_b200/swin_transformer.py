@@ -349,6 +349,17 @@ class BasicLayer(nn.Module):
             return pend[0].float()
         return x if pend is None else ops.residual_add(x, *pend)
 
+    def forward_with_features(self, x: Tensor):
+        """models/swin_transformer.py:483-490: x [B, L, C] -> (x after the downsample, [output of every block]), fp32."""
+        x, fea = x.float(), []
+        for blk in self.blocks:
+            x, pend = blk.fused(x, None)
+            x = ops.residual_add(x, *pend)
+            fea.append(x)
+        if self.downsample is not None:
+            x = self.downsample(x)
+        return x, fea
+
 
 class PatchEmbed(nn.Module):
     def __init__(self, img_size=224, patch_size=4, in_chans=3, embed_dim=96, norm_layer=None):
@@ -491,6 +502,41 @@ class SwinTransformer(nn.Module):
             probs = [[1.0 - blk.drop_prob] for layer in self.layers for blk in layer.blocks for _ in range(2)]
             t = cache[device] = torch.tensor(probs, dtype=torch.float32).to(device)
         return t
+
+    def forward_return_n_last_blocks(self, x: Tensor, n: int = 1, return_patch_avgpool: bool = False, depth=[]):
+        """models/swin_transformer.py:799-837 (eval_linear.py's probe features): fp32 [B, sum C_i], the token means of
+        the outputs of the last n blocks in execution order; outputs of last-stage blocks go through the final norm
+        first.  return_patch_avgpool is ignored, as in the reference.  `depth` must equal the model's depths.
+
+        Runs the fused path of forward_features: only a tapped block's output is materialised (residual_add), and the
+        stream continues from it; the last block's normed output is the final add+LN output itself."""
+        depths = [len(layer.blocks) for layer in self.layers]
+        if [int(d) for d in depth] != depths:
+            raise ValueError(f"depth {list(depth)} does not match the model's depths {depths}")
+        total = sum(depths)
+        if not 1 <= int(n) <= total:
+            raise ValueError(f"n must be in [1, {total}], got {n}")
+        start, last = total - int(n), len(self.layers) - 1
+        cc = _CastCache()
+        x = self.patch_embed(x)
+        pend, out, b = None, [], 0
+        for i, layer in enumerate(self.layers):
+            for j, blk in enumerate(layer.blocks):
+                x, pend = blk.fused(x, pend, cc)
+                if b >= start and not (i == last and j == len(layer.blocks) - 1):
+                    x, pend = ops.residual_add(x, *pend), None
+                    y = ops.LayerNormFn.apply(x, self.norm.weight, self.norm.bias, self.norm.eps, False) if i == last else x
+                    out.append(ops.TokenMeanFn.apply(y))
+                b += 1
+            if layer.downsample is not None:
+                if pend is not None:
+                    x = ops.residual_add(x, *pend)
+                x, pend = None, (layer.downsample.fused(x, cc), None, None)
+        delta, keep, dbias = pend if pend is not None else (None, None, None)
+        _, x_region = ops.add_layer_norm(x, delta, keep, self.norm.weight, self.norm.bias, self.norm.eps,
+                                         y_bf16=False, delta_bias=dbias)
+        out.append(ops.TokenMeanFn.apply(x_region))
+        return torch.cat(out, dim=-1)
 
     def forward_feature_maps(self, x: Tensor):
         d = self.use_dense_prediction

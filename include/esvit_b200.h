@@ -197,6 +197,25 @@ int esvit_adamw_ema_multi(void* const* params, const void* const* grads, void* c
                           const long long* numel, int n, const float* hyper, float* state, const double* sumsq,
                           void* stream);
 
+/* ---- exact weighted k-NN classifier over frozen features ---------------------------------------- eval_knn.py:193-232
+ * knn_prep: xb bf16 [R_pad, D] = bf16(x fp32 [R, D]) with rows >= R zero; norm fp32 [R] = ||x_r||; max_norm fp32 [1]
+ *   ACCUMULATED as the maximum norm (integer atomicMax on its bit pattern; caller zero-fills).  D % 8 == 0.
+ * knn_select: per test row r (rows int32 [nrows] or NULL = rows 0..nrows-1): S bf16 [., ld] = a . b^T from
+ *   esvit_gemm_bf16; a fp32 [., D] test rows with norms a_norm; b fp32 [N, D] train rows with max norm max_norm[0].
+ *   Finds the k-th largest bf16 value tau of S[r, 0:N], collects the columns with S >= tau - 2 delta_r
+ *   (delta_r = (3u + 4u^2 + D 2^-23) a_norm[r] max_norm, u = 2^-8) into cand_idx / cand_val [nrows, cap] (scratch),
+ *   rescores them in fp32 and writes the exact fp32 top-k by (value desc, index asc) to sims fp32 [., k] and idx int64
+ *   [., k].  count int32 [.] receives the candidate count; rows with count > cap are not written (rerun with cap >= count).
+ * knn_vote: per test row, scores[c] = sum of exp(sims / T) over the neighbours of train class c (rank order); hits int64
+ *   [2] ACCUMULATES (top-1, top-5) hits of test_labels by (score desc, class asc).  num_classes <= 11264. */
+int esvit_knn_prep(const float* x, void* xb, float* norm, float* max_norm, long long R, long long R_pad, int D,
+                   void* stream);
+int esvit_knn_select(const void* S, long long ld, const float* a, const float* b, const float* a_norm,
+                     const float* max_norm, const int* rows, int nrows, int N, int D, int k, int cap, int* cand_idx,
+                     float* cand_val, int* count, float* sims, long long* idx, void* stream);
+int esvit_knn_vote(const float* sims, const long long* idx, const long long* train_labels, const long long* test_labels,
+                   long long M, int k, float T, int num_classes, long long* hits, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
