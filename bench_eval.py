@@ -2,6 +2,7 @@
 
     python bench_eval.py probe   # forward_return_n_last_blocks(x, 4, False, depths), Swin-T W7, 224^2, B = 128
     python bench_eval.py knn     # knn_classifier on synthetic ImageNet-shaped features, k in {10, 20, 100, 200}
+    python bench_eval.py attn    # forward_selfattention(x, n=2), Swin-T W7, 224^2, B = 1 and 64 (analyze_models.py)
 
 probe: images/s of the CUDA path against the unmodified reference modules (oracle/_ref/, fp32, what eval_linear.py runs)
 on the same GPU and the same seeded weights, with the rel-L2 difference of their outputs.
@@ -11,6 +12,11 @@ unmodified eval_knn.knn_classifier (AST-extracted from oracle/_ref/eval_knn.py, 
 first --ref-test-rows test rows, with the top-1 / top-5 agreement and neighbour disagreements on those rows; the largest
 candidate count and the rerun rows; GEMM TFLOP/s against 989 (dense bf16) and select bytes/s against 3.35 TB/s, computed
 from shapes.
+
+attn: images/s of forward_selfattention(x, 2) against the unmodified reference modules (fp32, same seeded weights), the
+rel-L2 and max-abs difference of every map, and the probability kernel's time per image (CUDA events around every
+esvit_window_attn_probs launch) with its bytes/s against 3.35 TB/s; the bytes are the maps written plus the q/k rows read,
+computed from shapes.
 
 Writes nothing in the tree; card name, power limit and SM clocks are read in the same run.
 """
@@ -93,6 +99,61 @@ def probe(args) -> dict:
     return res
 
 
+def attn(args) -> dict:
+    from esvit_b200 import _lib
+    from esvit_b200.swin_transformer import SwinTransformer
+    from oracle import golden as GD
+    from oracle import reference_import as R
+    from oracle import swin as S
+    spec = dict(S.SWIN_T_W7)
+    m = SwinTransformer(img_size=224, num_classes=0, drop_path_rate=0.0, norm_layer=partial(nn.LayerNorm, eps=1e-6), **spec)
+    sd = GD.seeded_state_dict(GD.recipe(m.state_dict()), 0)
+    m.load_state_dict(sd)
+    m = m.cuda().eval()
+    ref = None
+    if R.available():
+        ns = R.load()
+        ref = ns.SwinTransformer(img_size=224, in_chans=3, num_classes=0, embed_dim=spec["embed_dim"],
+                                 depths=list(spec["depths"]), num_heads=list(spec["num_heads"]),
+                                 window_size=spec["window_size"], drop_path_rate=0.0,
+                                 norm_layer=partial(nn.LayerNorm, eps=1e-6))
+        ref.load_state_dict(sd)
+        ref = ref.cuda().eval()
+    res = {"mode": "attn", "arch": "swin_tiny_w7", "n": 2, "per_batch": {}}
+    for B in [int(b) for b in args.batches.split(",")]:
+        x = torch.randn(B, 3, 224, 224, generator=torch.Generator().manual_seed(1)).cuda()
+        with torch.no_grad():
+            t = _time(lambda: m.forward_selfattention(x, 2), args.steps, args.warmup)
+            _lib.reset_counters()
+            _lib.time_entry_point("esvit_window_attn_probs")
+            out = m.forward_selfattention(x, 2)
+            torch.cuda.synchronize()
+            _lib.time_entry_point(None)
+            calls = _lib.timed_results()
+        k_s = sum(c["ms"] for c in calls) / 1e3
+        k_bytes = sum(c["windows"] * c["nH"] * c["ws"] ** 4 * 4 + c["tokens"] * 2 * c["C"] * 2 for c in calls)
+        r = {"esvit_b200": {"s_per_batch": t, "images_per_s": B / t}, "maps": len(out),
+             "map_bytes_per_image": sum(o.numel() * 4 for o in out) / B,
+             "probs_kernel": {"launches": len(calls), "s_per_image": k_s / B, "bytes_per_image": k_bytes / B,
+                              "tbps": k_bytes / k_s / 1e12, "share_of_3.35": k_bytes / k_s / 1e12 / PEAK_HBM_TBPS}}
+        if ref is not None:
+            with torch.no_grad():
+                tr = _time(lambda: ref.forward_selfattention(x, 2), args.steps, args.warmup)
+                ro = ref.forward_selfattention(x, 2)
+            assert [o.shape for o in out] == [o.shape for o in ro]
+            num = sum(float((a.double() - b.double()).norm() ** 2) for a, b in zip(out, ro))
+            den = sum(float(b.double().norm() ** 2) for b in ro)
+            r["reference_fp32"] = {"s_per_batch": tr, "images_per_s": B / tr}
+            r["speedup"] = tr / t
+            r["rel_l2"] = (num / den) ** 0.5
+            r["max_abs"] = max(float((a - b).abs().max()) for a, b in zip(out, ro))
+        else:
+            r["reference_fp32"] = "oracle/_ref not installed"
+        res["per_batch"][B] = r
+        del out
+    return res
+
+
 def knn(args) -> dict:
     from esvit_b200 import _lib
     from esvit_b200 import knn as K
@@ -159,8 +220,9 @@ def knn(args) -> dict:
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("mode", choices=["probe", "knn"])
+    ap.add_argument("mode", choices=["probe", "knn", "attn"])
     ap.add_argument("--batch", type=int, default=128)
+    ap.add_argument("--batches", default="1,64", help="attn: batch sizes")
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--train-rows", type=int, default=1281167)
@@ -177,7 +239,7 @@ def main():
         sys.exit("bench_eval.py needs a CUDA device")
     torch.backends.cuda.matmul.allow_tf32 = False  # the reference arms run fp32
     before = card()
-    res = probe(args) if args.mode == "probe" else knn(args)
+    res = {"probe": probe, "knn": knn, "attn": attn}[args.mode](args)
     res["card"] = before
     res["card_after"] = card()
     print(json.dumps(res))

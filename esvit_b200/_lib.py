@@ -30,6 +30,7 @@ SIGNATURES = {
     "esvit_window_attn_expand_bias": [P, P, I, I, P],
     "esvit_window_attn_fwd": [P, P, P, P, I, P, P, I, I, I, I, I, I, I, F, P],
     "esvit_window_attn_bwd": [P, P, P, P, I, P, P, P, P, P, P, I, I, I, I, I, I, I, F, P],
+    "esvit_window_attn_probs": [P, P, P, P, I, P, I, I, I, I, I, I, I, F, P],
     "esvit_gemm_bias_act": [P, P, P, P, P, L, I, I, I, P],
     "esvit_gemm_mul_colsum": [P, P, P, P, P, P, L, I, I, P],
     "esvit_gemm_bf16": [P, P, P, P, P, L, I, I, I, I, I, I, P],
@@ -121,6 +122,7 @@ _META = {
     "esvit_dino_ce_bwd": lambda a: {"rows": int(a[-3]), "K": int(a[-2])},
     "esvit_window_attn_bwd": lambda a: _attn_meta(a),
     "esvit_window_attn_fwd": lambda a: _attn_meta(a),
+    "esvit_window_attn_probs": lambda a: _attn_meta(a),
     "esvit_gemm_bias_act": lambda a: {"M": int(a[5]), "N": int(a[6]), "K": int(a[7])},
     "esvit_gemm_mul_colsum": lambda a: {"M": int(a[6]), "N": int(a[7]), "K": int(a[8])},
     "esvit_gemm_bf16": lambda a: {"M": int(a[5]), "N": int(a[6]), "K": int(a[7]), "b_mn": int(a[9]), "act": int(a[10]),

@@ -19,12 +19,14 @@
 //
 // Math: bf16 mma.sync m16n8k16 with fp32 accumulate; softmax in fp32 registers; P rounded to bf16 for PV
 // (same as the reference under autocast).  head_dim is 32 in every Swin variant.
-// The backward recomputes P from the saved log-sum-exp (no [B_, nH, N, N] tensor is saved).
+// The backward recomputes P from the saved log-sum-exp (no [B_, nH, N, N] tensor is saved).  esvit_window_attn_probs
+// (window_attn_probs.cuh) writes P itself, for SwinTransformer.forward_selfattention.
 #include <cstdlib>
 
 #include "wa_common.cuh"
 #include "window_attn7.cuh"
 #include "window_attn14.cuh"
+#include "window_attn_probs.cuh"
 
 namespace wa {
 
@@ -148,6 +150,41 @@ ESVIT_API int esvit_window_attn_bwd(const void* qkv, const void* qkv_bias, const
       wa::window_attn_bwd14_kernel<false><<<grid, wa::T14, smem, st>>>(q, qb, bias_table, (const bf16*)out, (const bf16*)dout,
                                                                        lse, (bf16*)dqkv, bias_ws, dqkv_bias, g, scale, nwin);
     wa::fold_dbias14_kernel<<<dim3(27, nH), 192, 0, st>>>(bias_ws, dbias_table, nH);
+  }
+  ESVIT_LAUNCH_CHECK();
+}
+
+// probs fp32 [B*nWy*nWx, nH, ws*ws, ws*ws] is fully written: the softmax of every (window, head) of the call, padded slots
+// included, windows of the frame rolled by -shift (the reference's window_partition order).  Inputs as in
+// esvit_window_attn_fwd; nothing else is written (ws 7 with bias_ready = 0 expands the table into bias_ws first).
+ESVIT_API int esvit_window_attn_probs(const void* qkv, const void* qkv_bias, const float* bias_table, float* bias_ws,
+                                      int bias_ready, float* probs, int B, int H, int W, int C, int nH, int ws,
+                                      int shift, float scale, void* stream) {
+  wa::Geo g;
+  if (!wa::make_geo(g, B, H, W, C, nH, ws, shift) || !qkv || !qkv_bias || !bias_table || !probs) return ESVIT_ERR_BAD_ARG;
+  const int nwin = B * g.nWy * g.nWx;
+  cudaStream_t st = (cudaStream_t)stream;
+  const bf16* q = (const bf16*)qkv;
+  const bf16* qb = (const bf16*)qkv_bias;
+  if (ws == 7) {
+    if (!bias_ws) return ESVIT_ERR_BAD_ARG;
+    if (!bias_ready) wa::expand_bias7_kernel<<<nH, 256, 0, st>>>(bias_table, bias_ws, nH);
+    const size_t smem = wa::probs7_smem();
+    const dim3 grid(nH, wa::windows_grid(nwin, nH, 16));
+    if (shift > 0)
+      wa::window_attn_probs7_kernel<true><<<grid, 128, smem, st>>>(q, qb, bias_ws, probs, g, scale, nwin);
+    else
+      wa::window_attn_probs7_kernel<false><<<grid, 128, smem, st>>>(q, qb, bias_ws, probs, g, scale, nwin);
+  } else {
+    const size_t smem = wa::probs14_smem();
+    cudaError_t e = wa::opt_in_smem(wa::window_attn_probs14_kernel<true>, smem);
+    if (e == cudaSuccess) e = wa::opt_in_smem(wa::window_attn_probs14_kernel<false>, smem);
+    if (e != cudaSuccess) return (int)e;
+    const dim3 grid(nH, wa::windows_grid(nwin, nH, 2));
+    if (shift > 0)
+      wa::window_attn_probs14_kernel<true><<<grid, wa::T14, smem, st>>>(q, qb, bias_table, probs, g, scale, nwin);
+    else
+      wa::window_attn_probs14_kernel<false><<<grid, wa::T14, smem, st>>>(q, qb, bias_table, probs, g, scale, nwin);
   }
   ESVIT_LAUNCH_CHECK();
 }

@@ -43,8 +43,9 @@ __device__ __forceinline__ void zero_pad_rows14(bf16* tiles) {
   }
 }
 
-// async gather of the q/k/v rows of one window into [Q | K | V] tiles; padded slots get the bf16 qkv bias from
-// registers (see window_attn7.cuh: a global read would hammer one cache line from thousands of CTAs)
+// async gather of the q/k/v rows of one window into [Q | K | V] tiles ([Q | K] for NPART = 2); padded slots get the
+// bf16 qkv bias from registers (see window_attn7.cuh: a global read would hammer one cache line from thousands of CTAs)
+template <int NPART = 3>
 __device__ __forceinline__ void issue14(const Geo& g, int win, int h, const bf16* __restrict__ qkv,
                                         const uint4 (&bchunk)[3], bf16* tiles, int* tok, int* rid) {
   const int wx = win % g.nWx, wy = (win / g.nWx) % g.nWy, b = win / (g.nWx * g.nWy);
@@ -59,11 +60,11 @@ __device__ __forceinline__ void issue14(const Geo& g, int win, int h, const bf16
       bf16* dst = tiles + row * LD + c16 * 8;
       if (tk < 0) {
 #pragma unroll
-        for (int part = 0; part < 3; part++) *reinterpret_cast<uint4*>(dst + part * TILE14) = bchunk[part];
+        for (int part = 0; part < NPART; part++) *reinterpret_cast<uint4*>(dst + part * TILE14) = bchunk[part];
       } else {
         const bf16* src = qkv + (long long)tk * 3 * g.C + h * HD + c16 * 8;
 #pragma unroll
-        for (int part = 0; part < 3; part++) cp_async16(dst + part * TILE14, src + part * g.C, 16);
+        for (int part = 0; part < NPART; part++) cp_async16(dst + part * TILE14, src + part * g.C, 16);
       }
       if (c16 == 0) {
         tok[row] = tk;

@@ -33,11 +33,12 @@ __global__ void __launch_bounds__(256) expand_bias7_kernel(const float* __restri
   }
 }
 
-// Issue the async gathers of one window into a pipeline stage: tiles [Q | K | V] (+ [dO | O] and lse for BWD).
+// Issue the async gathers of one window into a pipeline stage: tiles [Q | K | V] (+ [dO | O] and lse for BWD); NPART = 2
+// gathers [Q | K] only.
 // Padded slots hold the qkv bias of this head: every thread keeps ITS three 16-byte bias chunks (q,k,v at its c16) in
 // registers and stores them to shared memory directly - gathering them from global memory made thousands of CTAs hammer
 // the same few cache lines (local crops: 5x slower gathers than global crops with the same window count).
-template <bool BWD, int NTHREADS = 128>
+template <bool BWD, int NTHREADS = 128, int NPART = 3>
 __device__ __forceinline__ void issue7(const Geo& g, int win, int h, const bf16* __restrict__ qkv,
                                        const uint4 (&bchunk)[3], const bf16* __restrict__ dout,
                                        const bf16* __restrict__ out, const float* __restrict__ lse, bf16* tiles,
@@ -56,11 +57,11 @@ __device__ __forceinline__ void issue7(const Geo& g, int win, int h, const bf16*
     const int nbytes = (t < NT && g.dbg != 1) ? 16 : 0;  // slots >= 49: zero fill (dbg 1: no global reads at all)
     if (t < NT && tk < 0) {
 #pragma unroll
-      for (int part = 0; part < 3; part++)
+      for (int part = 0; part < NPART; part++)
         *reinterpret_cast<uint4*>(tiles + part * TILE7 + t * LD + c16 * 8) = bchunk[part];
     } else {
 #pragma unroll
-      for (int part = 0; part < 3; part++)
+      for (int part = 0; part < NPART; part++)
         cp_async16(tiles + part * TILE7 + t * LD + c16 * 8, src_row + part * g.C, nbytes);
     }
     if (BWD) {

@@ -579,6 +579,32 @@ class TokenMeanGroupsFn(Function):
         return d, None
 
 
+@torch.no_grad()
+def window_attention_probs(qkv: Tensor, qkv_bias: Tensor, bias_table: Tensor, H: int, W: int, num_heads: int, ws: int,
+                           shift: int, scale: float, bias_exp: Optional[Tensor] = None) -> Tensor:
+    """The attention probabilities of the WindowAttentionFn call with the same arguments, fp32
+    [B*nWy*nWx, nH, ws*ws, ws*ws] in the reference's layout (the `attn` that WindowAttention.forward returns,
+    models/swin_transformer.py:141-152): windows of the padded frame rolled by -shift, rows and columns of padded slots
+    included.  Not differentiable."""
+    qkv = _chk(qkv, BF16, "qkv")
+    qkv_bias = _chk(qkv_bias, F32, "qkv_bias")
+    bias_table = _chk(bias_table.detach(), F32, "relative_position_bias_table")
+    B, L, C3 = qkv.shape
+    if L != H * W:
+        raise ValueError(f"qkv has {L} tokens per sample, expected H * W = {H * W}")
+    C = C3 // 3
+    qb = shadow.lookup(qkv_bias)
+    if qb is None:
+        qb = qkv_bias.detach().to(BF16)
+    nwin = B * (-(-H // ws)) * (-(-W // ws))
+    probs = torch.empty(nwin, num_heads, ws * ws, ws * ws, dtype=F32, device=qkv.device)
+    ready = 1 if (bias_exp is not None and ws == 7) else 0
+    bws = bias_exp if ready else torch.empty(num_heads * ATTN_WS_FLOATS, dtype=F32, device=qkv.device)
+    _lib.call("esvit_window_attn_probs", _p(qkv), _p(qb), _p(bias_table), _p(bws), ready, _p(probs), B, H, W, C,
+              num_heads, ws, shift, scale, _stream())
+    return probs
+
+
 def expand_rel_pos_bias(bias_table: Tensor, num_heads: int, ws: int) -> Optional[Tensor]:
     """ws = 7: the rel-pos bias table expanded ONCE for all attention calls (both crop groups, forward and backward) that
     use it this step -> fp32 [nH*4096] to pass as WindowAttentionFn's bias_exp; ws = 14: None (staged per CTA)."""

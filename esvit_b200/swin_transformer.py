@@ -194,14 +194,19 @@ class WindowAttention(nn.Module):
         self.proj = nn.Linear(dim, dim)
         _trunc_normal_(self.relative_position_bias_table, std=.02)
 
-    def attend(self, y: Tensor, H: int, W: int, shift: int, cc: Optional[_CastCache] = None) -> Tensor:
+    def attend(self, y: Tensor, H: int, W: int, shift: int, cc: Optional[_CastCache] = None,
+               maps: Optional[List[Tensor]] = None) -> Tensor:
         """y = norm1(x) bf16 [B, H*W, C] in token order -> proj(attention) bf16 [B, H*W, C]; proj.bias gets its gradient
-        from the residual-add kernel the caller routes it through."""
+        from the residual-add kernel the caller routes it through.  maps: a list to append the attention probabilities
+        to (ops.window_attention_probs, fp32 [B*nW, nH, N, N]), or None."""
         qkv = _lin_c(y, self.qkv, cc)
         ws = self.window_size[0]
         bexp = None if cc is None else cc.expanded_bias(self.relative_position_bias_table, self.num_heads, ws)
         a = ops.WindowAttentionFn.apply(qkv, self.qkv.bias, self.relative_position_bias_table, H, W, self.num_heads,
                                         ws, shift, float(self.scale), bexp)
+        if maps is not None:
+            maps.append(ops.window_attention_probs(qkv, self.qkv.bias, self.relative_position_bias_table, H, W,
+                                                   self.num_heads, ws, shift, float(self.scale), bexp))
         return _lin_c(a, self.proj, cc)
 
     def attend_groups(self, y: Tensor, grp, shift: int, cc: Optional[_CastCache] = None) -> Tensor:
@@ -242,14 +247,14 @@ class SwinTransformerBlock(nn.Module):
         self.norm2 = norm_layer(dim)
         self.mlp = Mlp(dim, int(dim * mlp_ratio), act_layer=act_layer, drop=drop)
 
-    def fused(self, x: Tensor, pending, cc: Optional[_CastCache] = None):
+    def fused(self, x: Tensor, pending, cc: Optional[_CastCache] = None, maps: Optional[List[Tensor]] = None):
         """(x fp32 [B,L,C], pending=(delta bf16, keep, delta_bias) or None) -> (x, pending): the MLP branch's
-        residual add (and fc2 bias) is deferred into the next fused add+LN."""
+        residual add (and fc2 bias) is deferred into the next fused add+LN.  maps: see WindowAttention.attend."""
         delta, keep, dbias = pending if pending is not None else (None, None, None)
         B, L, C = (x if x is not None else delta).shape  # x None: the stream starts as fp32(delta) (after PatchMerging)
         H = W = int(math.sqrt(L))
         x, y = ops.add_layer_norm(x, delta, keep, self.norm1.weight, self.norm1.bias, self.norm1.eps, delta_bias=dbias)
-        a = self.attn.attend(y, H, W, self.shift_size, cc)
+        a = self.attn.attend(y, H, W, self.shift_size, cc, maps)
         k1, k2 = drop_path_keeps(B, self.drop_prob, self.training, x.device, cc, id(self))
         x, y = ops.add_layer_norm(x, a, k1, self.norm2.weight, self.norm2.bias, self.norm2.eps,
                                   delta_bias=self.attn.proj.bias)
@@ -320,11 +325,13 @@ class BasicLayer(nn.Module):
                                  norm_layer=norm_layer) for i in range(depth)])
         self.downsample = downsample(input_resolution, dim=dim, norm_layer=norm_layer) if downsample else None
 
-    def fused(self, x: Optional[Tensor], cc: Optional[_CastCache] = None, pend=None):
+    def fused(self, x: Optional[Tensor], cc: Optional[_CastCache] = None, pend=None,
+              maps: Optional[List[Tensor]] = None):
         """(x fp32 or None, pend) -> (x, pend).  After a downsample the stream is handed on as (None, (merged bf16, None,
-        None)): the next stage's first add+LN turns it into the fp32 residual."""
+        None)): the next stage's first add+LN turns it into the fp32 residual.  maps: a list to append every block's
+        attention probabilities to, or None."""
         for blk in self.blocks:
-            x, pend = blk.fused(x, pend, cc)
+            x, pend = blk.fused(x, pend, cc, maps)
         if self.downsample is not None:
             x = ops.residual_add(x, *pend)
             return None, (self.downsample.fused(x, cc), None, None)
@@ -344,7 +351,16 @@ class BasicLayer(nn.Module):
         return x, pend, grp
 
     def forward(self, x: Tensor) -> Tensor:
-        x, pend = self.fused(x.float())
+        return self._forward(x, None)
+
+    def forward_with_attention(self, x: Tensor):
+        """models/swin_transformer.py:492-499: x [B, L, C] -> (x after the downsample, [attention probabilities of
+        every block, fp32 [B*nW, nH, N, N]]).  The probabilities do not require grad."""
+        maps = []
+        return self._forward(x, maps), maps
+
+    def _forward(self, x: Tensor, maps: Optional[List[Tensor]]) -> Tensor:
+        x, pend = self.fused(x.float(), maps=maps)
         if x is None:
             return pend[0].float()
         return x if pend is None else ops.residual_add(x, *pend)
@@ -537,6 +553,45 @@ class SwinTransformer(nn.Module):
                                          y_bf16=False, delta_bias=dbias)
         out.append(ops.TokenMeanFn.apply(x_region))
         return torch.cat(out, dim=-1)
+
+    def forward_selfattention(self, x: Tensor, n: int = 1):
+        """models/swin_transformer.py:766-778 (analyze_models.py's attention maps): images fp32 [B, 3, S, S] -> the last
+        block's attention probabilities if n == 1, else the list of every block's in execution order.  Each is fp32
+        [B*nW, nH, N, N] with the block's window (N = ws*ws) and windows in the reference's window_partition order of
+        the padded, rolled map; rows and columns of padded slots are included."""
+        if x.dim() != 4 or x.shape[2] != x.shape[3] or x.shape[2] % 4 != 0:
+            raise ValueError(f"expected square images [B, 3, S, S] with S a multiple of 4, got {tuple(x.shape)}")
+        x = self.patch_embed(x)
+        if n == 1:
+            return self.forward_last_selfattention(x)
+        return self.forward_all_selfattention(x)
+
+    def _check_tokens(self, x: Tensor) -> Tensor:
+        side = math.isqrt(x.shape[1]) if x.dim() == 3 else 0
+        if x.dim() != 3 or side * side != x.shape[1] or x.shape[2] != self.embed_dim:
+            raise ValueError(f"expected patch-embedded tokens [B, S*S, {self.embed_dim}], got {tuple(x.shape)}")
+        return x.float()
+
+    @torch.no_grad()
+    def forward_last_selfattention(self, x: Tensor) -> Tensor:
+        """models/swin_transformer.py:780-787: patch-embedded tokens [B, L, C] -> the last block's probabilities.  Runs the
+        fused path of forward_features; only the last block computes its probabilities."""
+        x, pend, cc, maps = self._check_tokens(x), None, _CastCache(), []
+        for layer in self.layers[:-1]:
+            x, pend = layer.fused(x, cc, pend)
+        blocks = self.layers[-1].blocks
+        for i, blk in enumerate(blocks):
+            x, pend = blk.fused(x, pend, cc, maps if i == len(blocks) - 1 else None)
+        return maps[0]
+
+    @torch.no_grad()
+    def forward_all_selfattention(self, x: Tensor) -> List[Tensor]:
+        """models/swin_transformer.py:789-796: patch-embedded tokens [B, L, C] -> every block's probabilities in execution
+        order (sum(depths) tensors)."""
+        x, pend, cc, maps = self._check_tokens(x), None, _CastCache(), []
+        for layer in self.layers:
+            x, pend = layer.fused(x, cc, pend, maps)
+        return maps
 
     def forward_feature_maps(self, x: Tensor):
         d = self.use_dense_prediction

@@ -77,6 +77,12 @@ int esvit_window_attn_bwd(const void* qkv, const void* qkv_bias, const float* bi
                           const void* out, const void* dout, const float* lse, void* dqkv, float* dbias_table,
                           float* dqkv_bias, int B, int H, int W, int C, int nH, int ws, int shift, float scale,
                           void* stream);
+/* Attention probabilities (SwinTransformer.forward_selfattention, models/swin_transformer.py:766-796; softmax :141-147):
+ * probs fp32 [B*nWy*nWx, nH, ws*ws, ws*ws] fully written, window w = b*nWy*nWx + wy*nWx + wx of the padded frame rolled
+ * by -shift, slots row-major, rows and columns of padded slots included.  qkv / qkv_bias / bias_table / bias_ws /
+ * bias_ready as for fwd; the row max and sum are computed here (the forward saves no LSE for all-padding query tiles). */
+int esvit_window_attn_probs(const void* qkv, const void* qkv_bias, const float* bias_table, float* bias_ws, int bias_ready,
+                            float* probs, int B, int H, int W, int C, int nH, int ws, int shift, float scale, void* stream);
 
 /* ---- wgmma / TMA GEMM with fused epilogue --------------------------- nn.Linear + Mlp.act, models/swin_transformer.py:31-33
  * out[M,N] (bf16) = act(a[M,K] @ w[N,K]^T + bias[N]); act 0 = identity, 1 = exact GELU (then `pre`, if not NULL, gets
