@@ -58,6 +58,12 @@ SIGNATURES = {
     "esvit_center_ema": [P, P, F, F, P, I, P],
     "esvit_normalize_rows": [P, P, L, I, F, P],
     "esvit_region_match": [P, P, I, I, I, I, I, P, P, P],
+    "esvit_mhsa_fwd": [P, P, P, I, I, I, I, F, P],
+    "esvit_mhsa_bwd": [P, P, P, P, P, P, I, I, I, I, F, P],
+    "esvit_vit_patches": [P, P, I, I, I, P],
+    "esvit_vit_tokens_fwd": [P, P, P, P, I, I, I, P],
+    "esvit_vit_tokens_bwd": [P, P, P, P, P, I, I, I, I, P],
+    "esvit_vit_split": [P, P, P, I, I, I, I, P],
     "esvit_ema_multi": [P, P, P, I, D, P],
     "esvit_clip_multi": [P, P, I, F, P, P, P],
     "esvit_grad_sumsq_multi": [P, P, I, P, P],
@@ -136,6 +142,9 @@ _META = {
     "esvit_dino_ce_q_fwd": lambda a: {"rows": int(a[-3]), "K": int(a[-2])},
     "esvit_dino_ce_q_bwd": lambda a: {"rows": int(a[-3]), "K": int(a[-2])},
     "esvit_row_softmax_q": lambda a: {"rows": int(a[-3]), "K": int(a[-2])},
+    "esvit_mhsa_fwd": lambda a: {"B": int(a[3]), "L": int(a[4]), "C": int(a[5]), "nH": int(a[6])},
+    "esvit_mhsa_bwd": lambda a: {"B": int(a[6]), "L": int(a[7]), "C": int(a[8]), "nH": int(a[9])},
+    "esvit_vit_tokens_bwd": lambda a: {"B": int(a[-5]), "N": int(a[-4]), "D": int(a[-3])},
     "esvit_patch_embed_fwd": lambda a: {"B": int(a[-5]), "H": int(a[-4]), "W": int(a[-3]), "E": int(a[-2])},
     "esvit_patch_embed_bwd": lambda a: {"B": int(a[-5]), "H": int(a[-4]), "W": int(a[-3]), "E": int(a[-2])},
 }

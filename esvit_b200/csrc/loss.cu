@@ -252,64 +252,81 @@ __global__ void __launch_bounds__(256) normalize_rows_kernel(const float* __rest
   }
 }
 
-// CTA (b, iq): the teacher view's Tt normalised region features are staged once in shared memory; each warp
-// takes student tokens of every crop v != iq, computes the Tt cosine similarities (fp32, warp-reduced dot)
-// and keeps the FIRST maximal index (torch.max tie rule, main_esvit.py:736).
+// CTA (b, iq): the teacher view's Tg normalised region features stream through shared memory in chunks of TC rows
+// (one chunk whenever all Tg * P fit, which covers every Swin shape; ViT at Tg = 196 needs several); each warp takes
+// student tokens of every crop v != iq, computes the cosine similarities (fp32, warp-reduced dot) and keeps the FIRST
+// maximal index (torch.max tie rule, main_esvit.py:736).  Across chunks the running maximum and its index are kept in
+// shared memory per token; the dot order and the strict > are those of a single pass, so the indices do not depend on TC.
 //   sn rows: crop v<2 at (v*B + b)*Tg + i ; crop v>=2 at 2*B*Tg + ((v-2)*B + b)*Tl + i
 //   tn rows: (iq*B + b)*Tg + j
 //   idx out: int64 [2, ncrops, B, Tg] (unused slots untouched); trow out: int32 [Rs, 2] (-1 where v == iq)
 constexpr int RM_MAXV = 8;  // P <= 1024
 __global__ void __launch_bounds__(256) region_match_kernel(const float* __restrict__ sn, const float* __restrict__ tn,
-                                                           int B, int ncrops, int Tg, int Tl, int P,
+                                                           int B, int ncrops, int Tg, int Tl, int P, int TC,
                                                            long long* __restrict__ idx_out, int* __restrict__ trow) {
-  extern __shared__ float tsm[];  // [Tg][P]
+  extern __shared__ float tsm[];  // [TC][P], then (TC < Tg) the running maximum [per_img] and its index [per_img]
   const int b = blockIdx.x, iq = blockIdx.y;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
   const float* tb = tn + ((long long)iq * B + b) * Tg * P;
-  for (int i = threadIdx.x * 4; i < Tg * P; i += blockDim.x * 4)
-    *reinterpret_cast<float4*>(tsm + i) = *reinterpret_cast<const float4*>(tb + i);
-  __syncthreads();
   const int per_img = 2 * Tg + (ncrops - 2) * Tl;  // student tokens of image b over all crops
-  for (int tok = warp; tok < per_img; tok += nw) {
-    int v, i, T;
-    long long srow;
-    if (tok < 2 * Tg) {
-      v = tok / Tg; i = tok - v * Tg; T = Tg;
-      srow = ((long long)v * B + b) * Tg + i;
-    } else {
-      const int u = tok - 2 * Tg;
-      v = 2 + u / Tl; i = u - (v - 2) * Tl; T = Tl;
-      srow = 2LL * B * Tg + ((long long)(v - 2) * B + b) * Tl + i;
-    }
-    (void)T;
-    if (v == iq) {
-      if (lane == 0) trow[2 * srow + iq] = -1;
-      continue;
-    }
-    float4 sv[RM_MAXV];
-#pragma unroll
-    for (int k = 0; k < RM_MAXV; k++) {
-      const int c = (k * 32 + lane) * 4;
-      sv[k] = c < P ? *reinterpret_cast<const float4*>(sn + srow * P + c) : make_float4(0, 0, 0, 0);
-    }
-    float best = -INFINITY;
-    int besti = 0;
-    for (int j = 0; j < Tg; j++) {
-      float d = 0.f;
+  float* run_best = tsm + (long long)TC * P;
+  int* run_idx = reinterpret_cast<int*>(run_best + per_img);
+  for (int j0 = 0; j0 < Tg; j0 += TC) {
+    const int jn = min(TC, Tg - j0);
+    const bool last = j0 + jn >= Tg;
+    if (j0 > 0) __syncthreads();  // every warp is done with the previous chunk
+    for (int i = threadIdx.x * 4; i < jn * P; i += blockDim.x * 4)
+      *reinterpret_cast<float4*>(tsm + i) = *reinterpret_cast<const float4*>(tb + (long long)j0 * P + i);
+    __syncthreads();
+    for (int tok = warp; tok < per_img; tok += nw) {
+      int v, i;
+      long long srow;
+      if (tok < 2 * Tg) {
+        v = tok / Tg; i = tok - v * Tg;
+        srow = ((long long)v * B + b) * Tg + i;
+      } else {
+        const int u = tok - 2 * Tg;
+        v = 2 + u / Tl; i = u - (v - 2) * Tl;
+        srow = 2LL * B * Tg + ((long long)(v - 2) * B + b) * Tl + i;
+      }
+      if (v == iq) {
+        if (lane == 0 && last) trow[2 * srow + iq] = -1;
+        continue;
+      }
+      float4 sv[RM_MAXV];
 #pragma unroll
       for (int k = 0; k < RM_MAXV; k++) {
         const int c = (k * 32 + lane) * 4;
-        if (c < P) {
-          float4 tv = *reinterpret_cast<const float4*>(tsm + j * P + c);
-          d += (sv[k].x * tv.x + sv[k].y * tv.y) + (sv[k].z * tv.z + sv[k].w * tv.w);
+        sv[k] = c < P ? *reinterpret_cast<const float4*>(sn + srow * P + c) : make_float4(0, 0, 0, 0);
+      }
+      float best = -INFINITY;
+      int besti = 0;
+      if (j0 > 0) {
+        best = run_best[tok];
+        besti = run_idx[tok];
+      }
+      for (int j = 0; j < jn; j++) {
+        float d = 0.f;
+#pragma unroll
+        for (int k = 0; k < RM_MAXV; k++) {
+          const int c = (k * 32 + lane) * 4;
+          if (c < P) {
+            float4 tv = *reinterpret_cast<const float4*>(tsm + j * P + c);
+            d += (sv[k].x * tv.x + sv[k].y * tv.y) + (sv[k].z * tv.z + sv[k].w * tv.w);
+          }
+        }
+        d = warp_sum(d);
+        if (d > best) { best = d; besti = j0 + j; }
+      }
+      if (lane == 0) {
+        if (last) {
+          idx_out[(((long long)iq * ncrops + v) * B + b) * Tg + i] = besti;
+          trow[2 * srow + iq] = (iq * B + b) * Tg + besti;
+        } else {
+          run_best[tok] = best;
+          run_idx[tok] = besti;
         }
       }
-      d = warp_sum(d);
-      if (d > best) { best = d; besti = j; }
-    }
-    if (lane == 0) {
-      idx_out[(((long long)iq * ncrops + v) * B + b) * Tg + i] = besti;
-      trow[2 * srow + iq] = (iq * B + b) * Tg + besti;
     }
   }
 }
@@ -583,10 +600,17 @@ ESVIT_API int esvit_normalize_rows(const float* x, float* y, long long R, int P,
 ESVIT_API int esvit_region_match(const float* sn, const float* tn, int B, int ncrops, int Tg, int Tl, int P,
                                  long long* idx_out, int* trow, void* stream) {
   if (P % 4 != 0 || P > 128 * RM_MAXV || B <= 0 || ncrops < 2) return ESVIT_ERR_BAD_ARG;
-  const size_t smem = (size_t)Tg * P * sizeof(float);
-  if (smem > 220 * 1024) return ESVIT_ERR_BAD_ARG;
+  const size_t budget = 220 * 1024, row = (size_t)P * sizeof(float);
+  const size_t state = (size_t)(2 * Tg + (ncrops - 2) * Tl) * (sizeof(float) + sizeof(int));
+  int TC = Tg;  // all teacher rows in one chunk when they fit, else as many as fit beside the running arg-max state
+  size_t smem = (size_t)Tg * row;
+  if (smem > budget) {
+    if (state + row > budget) return ESVIT_ERR_BAD_ARG;
+    TC = (int)((budget - state) / row);
+    smem = (size_t)TC * row + state;
+  }
   cudaError_t e = cudaFuncSetAttribute(region_match_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
-  region_match_kernel<<<dim3(B, 2), 256, smem, (cudaStream_t)stream>>>(sn, tn, B, ncrops, Tg, Tl, P, idx_out, trow);
+  region_match_kernel<<<dim3(B, 2), 256, smem, (cudaStream_t)stream>>>(sn, tn, B, ncrops, Tg, Tl, P, TC, idx_out, trow);
   ESVIT_LAUNCH_CHECK();
 }

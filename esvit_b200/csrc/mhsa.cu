@@ -1,0 +1,415 @@
+// Whole-sequence multi-head self-attention at head dim 64 (the ViT / DeiT backbones), forward and backward.
+//
+// Reference: models/vision_transformer.py  Attention.forward :83-95
+//   qkv = Linear(x).reshape(B, N, 3, nH, 64)  ->  softmax(q k^T * scale) v  ->  .transpose(1, 2).reshape(B, N, C)
+//
+// qkv bf16 [B*L, 3C] token-major as the qkv GEMM writes it (bias included), channel order [q|k|v][head][64].
+// out bf16 [B*L, C] in the reference's (head, dim) channel order; lse fp32 [B, nH, L] (natural log) for the backward.
+//
+// One CTA = 4 warps = 64 query rows (16 per warp) of one (sequence, head); mma.sync m16n8k16 bf16 with fp32
+// accumulation, fp32 online softmax in the log2 domain, P rounded to bf16 for PV, K / V tiles of 64 keys double-buffered
+// through cp.async.  Rows / keys past L are zero-filled tiles: keys past L get a score of -inf (P = 0 exactly), queries
+// past L are computed and never stored.
+//
+// Backward (no floating-point atomics, so dq / dk / dv are bit-reproducible):
+//   prep   D[b,h,i] = sum_d dO * O
+//   dq     CTA = 64 queries: P = ex2(s' - lse'), dP = dO V^T, dS = P (dP - D), dQ = scale * dS K   (loop over key tiles)
+//   dkdv   CTA = 64 keys:    P^T, dV = P^T dO, dP^T = V dO^T, dS^T = P^T (dP^T - D), dK = scale * dS^T Q  (loop over queries)
+// Each output row is owned by exactly one warp.
+#include "wa_common.cuh"
+
+namespace mh {
+
+using wa::cp_async16;
+using wa::cp_async_commit;
+using wa::cp_async_wait;
+using wa::ex2;
+using wa::ldsm_x4;
+using wa::ldsm_x4_t;
+using wa::lg2;
+using wa::LN2;
+using wa::LOG2E;
+using wa::mma16816;
+
+constexpr int HD = 64;
+constexpr int LDS = 72;            // smem row stride (bf16): 144 B rows -> conflict-free ldmatrix
+constexpr int TILE = 64 * LDS;     // one 64-row tile
+constexpr int NTHR = 128;
+
+// async copy of a [64 rows x 64 bf16] tile whose row 0 starts at src (row stride ld elements); rows >= nvalid are zero
+__device__ __forceinline__ void load_tile(bf16* dst, const bf16* __restrict__ src, long long ld, int nvalid) {
+#pragma unroll
+  for (int k = 0; k < 4; k++) {
+    const int e = threadIdx.x + k * NTHR;  // 512 chunks of 16 B
+    const int r = e >> 3, c = (e & 7) * 8;
+    const bool ok = r < nvalid;
+    cp_async16(dst + r * LDS + c, src + (ok ? (long long)r * ld : 0) + c, ok ? 16 : 0);
+  }
+}
+
+// A fragments (16 rows x 64) of rows r0.. of a tile
+__device__ __forceinline__ void load_a(uint32_t (&a)[4][4], const bf16* t, int r0, int lane) {
+  const bf16* p = t + (r0 + (lane & 7) + ((lane >> 3) & 1) * 8) * LDS + (lane >> 4) * 8;
+#pragma unroll
+  for (int k = 0; k < 4; k++) ldsm_x4(a[k], p + k * 16);
+}
+
+// acc[nt] (16 x 8 per nt, 64 columns) = A (16 x 64) . T^T where T's rows are the 64 columns (k = the 64 dims)
+__device__ __forceinline__ void mma_abt(float (&acc)[8][4], const uint32_t (&a)[4][4], const bf16* t, int lane) {
+#pragma unroll
+  for (int nt = 0; nt < 8; nt++) {
+    acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
+    const bf16* p = t + (nt * 8 + (lane & 7)) * LDS + (lane >> 3) * 8;
+    uint32_t b[4];
+    ldsm_x4(b, p);
+    mma16816(acc[nt], a[0], b[0], b[1]);
+    mma16816(acc[nt], a[1], b[2], b[3]);
+    ldsm_x4(b, p + 32);
+    mma16816(acc[nt], a[2], b[0], b[1]);
+    mma16816(acc[nt], a[3], b[2], b[3]);
+  }
+}
+
+// o[dt] (16 x 64) += P (16 x 64, fp32 fragments rounded to bf16) . T where T is [64 rows (k) x 64 dims]
+__device__ __forceinline__ void mma_pt(float (&o)[8][4], const float (&p)[8][4], const bf16* t, int lane) {
+#pragma unroll
+  for (int kk = 0; kk < 4; kk++) {
+    uint32_t pa[4];
+    pa[0] = pack_bf162(p[2 * kk][0], p[2 * kk][1]);
+    pa[1] = pack_bf162(p[2 * kk][2], p[2 * kk][3]);
+    pa[2] = pack_bf162(p[2 * kk + 1][0], p[2 * kk + 1][1]);
+    pa[3] = pack_bf162(p[2 * kk + 1][2], p[2 * kk + 1][3]);
+    const bf16* vp = t + (kk * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * LDS + (lane >> 4) * 8;
+#pragma unroll
+    for (int d16 = 0; d16 < 4; d16++) {
+      uint32_t vb[4];
+      ldsm_x4_t(vb, vp + d16 * 16);
+      mma16816(o[2 * d16], pa, vb[0], vb[1]);
+      mma16816(o[2 * d16 + 1], pa, vb[2], vb[3]);
+    }
+  }
+}
+
+// 16 x 64 fp32 fragments -> bf16 rows (rA, rB) of dst (row stride ld), rows >= L skipped
+__device__ __forceinline__ void store_rows(bf16* __restrict__ dst, long long ld, const float (&o)[8][4], float s0,
+                                           float s1, int rA, int rB, int L, int lane) {
+#pragma unroll
+  for (int dt = 0; dt < 8; dt++) {
+    const int d = dt * 8 + (lane & 3) * 2;
+    if (rA < L) *reinterpret_cast<uint32_t*>(dst + (long long)rA * ld + d) = pack_bf162(o[dt][0] * s0, o[dt][1] * s0);
+    if (rB < L) *reinterpret_cast<uint32_t*>(dst + (long long)rB * ld + d) = pack_bf162(o[dt][2] * s1, o[dt][3] * s1);
+  }
+}
+
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(NTHR) mhsa_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out,
+                                                        float* __restrict__ lse, int L, int C, int nH, float c2) {
+  extern __shared__ __align__(16) unsigned char smraw[];
+  bf16* Qs = reinterpret_cast<bf16*>(smraw);  // [Q | K0 | V0 | K1 | V1]
+  const int q0 = blockIdx.x * 64, h = blockIdx.y, b = blockIdx.z;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long C3 = 3LL * C;
+  const bf16* base = qkv + (long long)b * L * C3 + h * HD;
+  load_tile(Qs, base + q0 * C3, C3, L - q0);
+  load_tile(Qs + TILE, base + C, C3, L);
+  load_tile(Qs + 2 * TILE, base + 2 * C, C3, L);
+  cp_async_commit();
+  const int nkt = (L + 63) / 64;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+  float o[8][4];
+#pragma unroll
+  for (int dt = 0; dt < 8; dt++) o[dt][0] = o[dt][1] = o[dt][2] = o[dt][3] = 0.f;
+  uint32_t qa[4][4];
+  for (int kt = 0; kt < nkt; kt++) {
+    const int st = kt & 1;
+    if (kt + 1 < nkt) {
+      bf16* nx = Qs + (1 + 2 * (st ^ 1)) * TILE;
+      load_tile(nx, base + C + (kt + 1) * 64 * C3, C3, L - (kt + 1) * 64);
+      load_tile(nx + TILE, base + 2 * C + (kt + 1) * 64 * C3, C3, L - (kt + 1) * 64);
+    }
+    cp_async_commit();
+    cp_async_wait<1>();
+    __syncthreads();
+    const bf16* Ks = Qs + (1 + 2 * st) * TILE;
+    if (kt == 0) load_a(qa, Qs, warp * 16, lane);
+    float s[8][4];
+    mma_abt(s, qa, Ks, lane);
+    const bool edge = kt * 64 + 64 > L;
+#pragma unroll
+    for (int nt = 0; nt < 8; nt++) {
+#pragma unroll
+      for (int i = 0; i < 4; i++) s[nt][i] *= c2;
+      if (edge) {
+        const int key = kt * 64 + nt * 8 + (lane & 3) * 2;
+        if (key >= L) s[nt][0] = s[nt][2] = -INFINITY;
+        if (key + 1 >= L) s[nt][1] = s[nt][3] = -INFINITY;
+      }
+    }
+    float mx0 = m0, mx1 = m1;
+#pragma unroll
+    for (int nt = 0; nt < 8; nt++) {
+      mx0 = fmaxf(mx0, fmaxf(s[nt][0], s[nt][1]));
+      mx1 = fmaxf(mx1, fmaxf(s[nt][2], s[nt][3]));
+    }
+    mx0 = quad_max(mx0);
+    mx1 = quad_max(mx1);  // finite: every key tile holds at least one key < L
+    const float a0 = ex2(m0 - mx0), a1 = ex2(m1 - mx1);
+    m0 = mx0;
+    m1 = mx1;
+    float r0 = 0.f, r1 = 0.f;
+#pragma unroll
+    for (int nt = 0; nt < 8; nt++) {
+      s[nt][0] = ex2(s[nt][0] - m0);
+      s[nt][1] = ex2(s[nt][1] - m0);
+      s[nt][2] = ex2(s[nt][2] - m1);
+      s[nt][3] = ex2(s[nt][3] - m1);
+      r0 += s[nt][0] + s[nt][1];
+      r1 += s[nt][2] + s[nt][3];
+    }
+    l0 = l0 * a0 + r0;
+    l1 = l1 * a1 + r1;
+#pragma unroll
+    for (int dt = 0; dt < 8; dt++) {
+      o[dt][0] *= a0; o[dt][1] *= a0;
+      o[dt][2] *= a1; o[dt][3] *= a1;
+    }
+    mma_pt(o, s, Ks + TILE, lane);
+    __syncthreads();  // the next iteration's copy overwrites this stage
+  }
+  cp_async_wait<0>();
+  l0 = quad_sum(l0);
+  l1 = quad_sum(l1);
+  const int rA = q0 + warp * 16 + (lane >> 2), rB = rA + 8;
+  store_rows(out + (long long)b * L * C + h * HD, C, o, __fdividef(1.f, l0), __fdividef(1.f, l1), rA, rB, L, lane);
+  if ((lane & 3) == 0) {
+    float* lp = lse + ((long long)b * nH + h) * L;
+    if (rA < L) lp[rA] = (m0 + lg2(l0)) * LN2;
+    if (rB < L) lp[rB] = (m1 + lg2(l1)) * LN2;
+  }
+}
+
+// D[b, h, i] = sum_d dO[b, i, h, d] * O[b, i, h, d]; one warp per token row, lanes over (head, dim pair)
+__global__ void __launch_bounds__(256) mhsa_bwd_prep_kernel(const bf16* __restrict__ out, const bf16* __restrict__ dout,
+                                                            float* __restrict__ dvec, int B, int L, int C, int nH) {
+  const int lane = threadIdx.x & 31;
+  const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (row >= (long long)B * L) return;
+  const int b = (int)(row / L), i = (int)(row - (long long)b * L);
+  for (int h = 0; h < nH; h++) {
+    const long long off = row * C + h * HD + lane * 2;
+    const float2 o = __bfloat1622float2(*reinterpret_cast<const bf162*>(out + off));
+    const float2 g = __bfloat1622float2(*reinterpret_cast<const bf162*>(dout + off));
+    const float d = warp_sum(o.x * g.x + o.y * g.y);
+    if (lane == 0) dvec[((long long)b * nH + h) * L + i] = d;
+  }
+}
+
+// dQ of 64 query rows; lse / dvec as the forward / prep kernels wrote them
+__global__ void __launch_bounds__(NTHR) mhsa_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
+                                                           const float* __restrict__ lse, const float* __restrict__ dvec,
+                                                           bf16* __restrict__ dqkv, int L, int C, int nH, float c2,
+                                                           float scale) {
+  extern __shared__ __align__(16) unsigned char smraw[];
+  bf16* Qs = reinterpret_cast<bf16*>(smraw);  // [Q | dO | K0 | V0 | K1 | V1]
+  const int q0 = blockIdx.x * 64, h = blockIdx.y, b = blockIdx.z;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long C3 = 3LL * C;
+  const bf16* base = qkv + (long long)b * L * C3 + h * HD;
+  load_tile(Qs, base + q0 * C3, C3, L - q0);
+  load_tile(Qs + TILE, dout + ((long long)b * L + q0) * C + h * HD, C, L - q0);
+  load_tile(Qs + 2 * TILE, base + C, C3, L);
+  load_tile(Qs + 3 * TILE, base + 2 * C, C3, L);
+  cp_async_commit();
+  const int rA = q0 + warp * 16 + (lane >> 2), rB = rA + 8;
+  const float* lp = lse + ((long long)b * nH + h) * L;
+  const float* dp = dvec + ((long long)b * nH + h) * L;
+  const float lA = rA < L ? lp[rA] * LOG2E : 0.f, lB = rB < L ? lp[rB] * LOG2E : 0.f;
+  const float DA = rA < L ? dp[rA] : 0.f, DB = rB < L ? dp[rB] : 0.f;
+  const int nkt = (L + 63) / 64;
+  float dq[8][4];
+#pragma unroll
+  for (int dt = 0; dt < 8; dt++) dq[dt][0] = dq[dt][1] = dq[dt][2] = dq[dt][3] = 0.f;
+  uint32_t qa[4][4], oa[4][4];
+  for (int kt = 0; kt < nkt; kt++) {
+    const int st = kt & 1;
+    if (kt + 1 < nkt) {
+      bf16* nx = Qs + (2 + 2 * (st ^ 1)) * TILE;
+      load_tile(nx, base + C + (kt + 1) * 64 * C3, C3, L - (kt + 1) * 64);
+      load_tile(nx + TILE, base + 2 * C + (kt + 1) * 64 * C3, C3, L - (kt + 1) * 64);
+    }
+    cp_async_commit();
+    cp_async_wait<1>();
+    __syncthreads();
+    const bf16* Ks = Qs + (2 + 2 * st) * TILE;
+    if (kt == 0) {
+      load_a(qa, Qs, warp * 16, lane);
+      load_a(oa, Qs + TILE, warp * 16, lane);
+    }
+    float p[8][4], g[8][4];
+    mma_abt(p, qa, Ks, lane);
+    mma_abt(g, oa, Ks + TILE, lane);
+    const bool edge = kt * 64 + 64 > L;
+#pragma unroll
+    for (int nt = 0; nt < 8; nt++) {
+      p[nt][0] = ex2(p[nt][0] * c2 - lA);
+      p[nt][1] = ex2(p[nt][1] * c2 - lA);
+      p[nt][2] = ex2(p[nt][2] * c2 - lB);
+      p[nt][3] = ex2(p[nt][3] * c2 - lB);
+      if (edge) {
+        const int key = kt * 64 + nt * 8 + (lane & 3) * 2;
+        if (key >= L) p[nt][0] = p[nt][2] = 0.f;
+        if (key + 1 >= L) p[nt][1] = p[nt][3] = 0.f;
+      }
+      p[nt][0] *= g[nt][0] - DA;
+      p[nt][1] *= g[nt][1] - DA;
+      p[nt][2] *= g[nt][2] - DB;
+      p[nt][3] *= g[nt][3] - DB;
+    }
+    mma_pt(dq, p, Ks, lane);
+    __syncthreads();
+  }
+  cp_async_wait<0>();
+  store_rows(dqkv + (long long)b * L * C3 + h * HD, C3, dq, scale, scale, rA, rB, L, lane);
+}
+
+// dK, dV of 64 key rows
+__global__ void __launch_bounds__(NTHR) mhsa_bwd_dkdv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
+                                                             const float* __restrict__ lse, const float* __restrict__ dvec,
+                                                             bf16* __restrict__ dqkv, int L, int C, int nH, float c2,
+                                                             float scale) {
+  extern __shared__ __align__(16) unsigned char smraw[];
+  bf16* Ks = reinterpret_cast<bf16*>(smraw);            // [K | V | Q0 | dO0 | Q1 | dO1]
+  float* stat = reinterpret_cast<float*>(Ks + 6 * TILE);  // [2 stages][lse' 64 | D 64]
+  const int k0 = blockIdx.x * 64, h = blockIdx.y, b = blockIdx.z;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long C3 = 3LL * C;
+  const bf16* base = qkv + (long long)b * L * C3 + h * HD;
+  const bf16* gbase = dout + (long long)b * L * C + h * HD;
+  const float* lp = lse + ((long long)b * nH + h) * L;
+  const float* dp = dvec + ((long long)b * nH + h) * L;
+  load_tile(Ks, base + C + k0 * C3, C3, L - k0);
+  load_tile(Ks + TILE, base + 2 * C + k0 * C3, C3, L - k0);
+  load_tile(Ks + 2 * TILE, base, C3, L);
+  load_tile(Ks + 3 * TILE, gbase, C, L);
+  cp_async_commit();
+  if (threadIdx.x < 64) {  // queries past L: lse' = +inf -> P = 0
+    const int q = threadIdx.x;
+    stat[q] = q < L ? lp[q] * LOG2E : INFINITY;
+    stat[64 + q] = q < L ? dp[q] : 0.f;
+  }
+  const int nqt = (L + 63) / 64;
+  float dk[8][4], dv[8][4];
+#pragma unroll
+  for (int dt = 0; dt < 8; dt++)
+#pragma unroll
+    for (int i = 0; i < 4; i++) dk[dt][i] = dv[dt][i] = 0.f;
+  uint32_t ka[4][4], va[4][4];
+  for (int qt = 0; qt < nqt; qt++) {
+    const int st = qt & 1;
+    if (qt + 1 < nqt) {
+      bf16* nx = Ks + (2 + 2 * (st ^ 1)) * TILE;
+      const int n0 = (qt + 1) * 64;
+      load_tile(nx, base + n0 * C3, C3, L - n0);
+      load_tile(nx + TILE, gbase + (long long)n0 * C, C, L - n0);
+      if (threadIdx.x < 64) {
+        const int q = n0 + threadIdx.x;
+        float* sn = stat + (st ^ 1) * 128;
+        sn[threadIdx.x] = q < L ? lp[q] * LOG2E : INFINITY;
+        sn[64 + threadIdx.x] = q < L ? dp[q] : 0.f;
+      }
+    }
+    cp_async_commit();
+    cp_async_wait<1>();
+    __syncthreads();
+    const bf16* Qs = Ks + (2 + 2 * st) * TILE;
+    const float* sl = stat + st * 128;
+    if (qt == 0) {
+      load_a(ka, Ks, warp * 16, lane);
+      load_a(va, Ks + TILE, warp * 16, lane);
+    }
+    float p[8][4], g[8][4];
+    mma_abt(p, ka, Qs, lane);         // S^T: keys x queries
+    mma_abt(g, va, Qs + TILE, lane);  // dP^T = V dO^T
+#pragma unroll
+    for (int nt = 0; nt < 8; nt++) {
+      const int q = nt * 8 + (lane & 3) * 2;
+      const float2 lq = *reinterpret_cast<const float2*>(sl + q);
+      p[nt][0] = ex2(p[nt][0] * c2 - lq.x);
+      p[nt][1] = ex2(p[nt][1] * c2 - lq.y);
+      p[nt][2] = ex2(p[nt][2] * c2 - lq.x);
+      p[nt][3] = ex2(p[nt][3] * c2 - lq.y);
+    }
+    mma_pt(dv, p, Qs + TILE, lane);   // dV += P^T dO
+#pragma unroll
+    for (int nt = 0; nt < 8; nt++) {
+      const int q = nt * 8 + (lane & 3) * 2;
+      const float2 dq = *reinterpret_cast<const float2*>(sl + 64 + q);
+      p[nt][0] *= g[nt][0] - dq.x;
+      p[nt][1] *= g[nt][1] - dq.y;
+      p[nt][2] *= g[nt][2] - dq.x;
+      p[nt][3] *= g[nt][3] - dq.y;
+    }
+    mma_pt(dk, p, Qs, lane);          // dK += dS^T Q
+    __syncthreads();
+  }
+  cp_async_wait<0>();
+  const int rA = k0 + warp * 16 + (lane >> 2), rB = rA + 8;
+  bf16* dst = dqkv + (long long)b * L * C3 + h * HD;
+  store_rows(dst + C, C3, dk, scale, scale, rA, rB, L, lane);
+  store_rows(dst + 2 * C, C3, dv, 1.f, 1.f, rA, rB, L, lane);
+}
+
+constexpr size_t FWD_SMEM = 5 * TILE * sizeof(bf16);
+constexpr size_t DQ_SMEM = 6 * TILE * sizeof(bf16);
+constexpr size_t DKDV_SMEM = 6 * TILE * sizeof(bf16) + 2 * 128 * sizeof(float);
+
+static bool ok_args(const void* a, const void* b, int B, int L, int C, int nH) {
+  return a && b && B >= 1 && B <= 65535 && L >= 1 && nH >= 1 && C == nH * HD && ((uintptr_t)a & 15) == 0 &&
+         ((uintptr_t)b & 15) == 0;
+}
+
+template <typename K>
+static cudaError_t opt_in(K kernel, size_t smem) {
+  return smem > 48 * 1024 ? cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
+                          : cudaSuccess;
+}
+
+}  // namespace mh
+
+ESVIT_API int esvit_mhsa_fwd(const void* qkv, void* out, float* lse, int B, int L, int C, int nH, float scale,
+                             void* stream) {
+  if (!mh::ok_args(qkv, out, B, L, C, nH) || !lse) return ESVIT_ERR_BAD_ARG;
+  const dim3 grid((L + 63) / 64, nH, B);
+  mh::mhsa_fwd_kernel<<<grid, mh::NTHR, mh::FWD_SMEM, (cudaStream_t)stream>>>(
+      (const bf16*)qkv, (bf16*)out, lse, L, C, nH, scale * mh::LOG2E);
+  ESVIT_LAUNCH_CHECK();
+}
+
+ESVIT_API int esvit_mhsa_bwd(const void* qkv, const void* out, const void* dout, const float* lse, float* dvec,
+                             void* dqkv, int B, int L, int C, int nH, float scale, void* stream) {
+  if (!mh::ok_args(qkv, dqkv, B, L, C, nH) || !mh::ok_args(out, dout, B, L, C, nH) || !lse || !dvec)
+    return ESVIT_ERR_BAD_ARG;
+  cudaError_t e = mh::opt_in(mh::mhsa_bwd_dq_kernel, mh::DQ_SMEM);
+  if (e == cudaSuccess) e = mh::opt_in(mh::mhsa_bwd_dkdv_kernel, mh::DKDV_SMEM);
+  if (e != cudaSuccess) return (int)e;
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long rows = (long long)B * L;
+  mh::mhsa_bwd_prep_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>((const bf16*)out, (const bf16*)dout, dvec, B, L, C,
+                                                                      nH);
+  const dim3 grid((L + 63) / 64, nH, B);
+  const float c2 = scale * mh::LOG2E;
+  mh::mhsa_bwd_dq_kernel<<<grid, mh::NTHR, mh::DQ_SMEM, st>>>((const bf16*)qkv, (const bf16*)dout, lse, dvec,
+                                                              (bf16*)dqkv, L, C, nH, c2, scale);
+  mh::mhsa_bwd_dkdv_kernel<<<grid, mh::NTHR, mh::DKDV_SMEM, st>>>((const bf16*)qkv, (const bf16*)dout, lse, dvec,
+                                                                  (bf16*)dqkv, L, C, nH, c2, scale);
+  ESVIT_LAUNCH_CHECK();
+}

@@ -20,6 +20,7 @@ import torch.distributed as dist
 from . import ops, utils
 from .losses import DDINOLoss, DINOLoss
 from .optim import FusedAdamWEMA
+from . import vision_transformer as vits
 from .swin_transformer import SwinTransformer
 from .vision_transformer import DINOHead
 
@@ -30,17 +31,29 @@ SWIN_SPECS = {
     "swin_base_w7": dict(embed_dim=128, depths=[2, 2, 18, 2], num_heads=[4, 8, 16, 32], window_size=7, drop_path_rate=0.2),
     "swin_base_w14": dict(embed_dim=128, depths=[2, 2, 18, 2], num_heads=[4, 8, 16, 32], window_size=14, drop_path_rate=0.2),
 }
+# ViT / DeiT (main_esvit.py:304-327): `vit_arch` names the factory in esvit_b200.vision_transformer
+VIT_SPECS = {
+    "deit_tiny_p16": dict(vit_arch="deit_tiny", patch_size=16, drop_path_rate=0.1),
+    "deit_small_p16": dict(vit_arch="deit_small", patch_size=16, drop_path_rate=0.1),
+    "deit_small_p8": dict(vit_arch="deit_small", patch_size=8, drop_path_rate=0.1),
+    "vit_base_p16": dict(vit_arch="vit_base", patch_size=16, drop_path_rate=0.1),
+}
 
 
 def build_network(spec: dict, out_dim: int, use_dense_prediction: bool, is_teacher: bool = False,
                   norm_last_layer: bool = True, img_size: int = 224, head_kwargs: Optional[dict] = None) -> nn.Module:
-    """What main_esvit.py:235-254 builds: Swin backbone (teacher: drop_path 0) + DINOHead(s) assigned to
-    ``.head`` / ``.head_dense``."""
+    """What main_esvit.py:235-254 (Swin) / :304-327 (ViT, a spec with `vit_arch`) builds: the backbone (teacher:
+    drop_path 0) + DINOHead(s) assigned to ``.head`` / ``.head_dense``."""
     spec = dict(spec)
     if is_teacher:
         spec["drop_path_rate"] = 0.0
-    net = SwinTransformer(img_size=img_size, in_chans=3, num_classes=0, patch_size=4, mlp_ratio=4., qkv_bias=True,
-                          norm_layer=partial(nn.LayerNorm, eps=1e-6), use_dense_prediction=use_dense_prediction, **spec)
+    vit_arch = spec.pop("vit_arch", None)
+    if vit_arch is not None:
+        net = vits.__dict__[vit_arch](img_size=[img_size], use_dense_prediction=use_dense_prediction, **spec)
+    else:
+        net = SwinTransformer(img_size=img_size, in_chans=3, num_classes=0, patch_size=4, mlp_ratio=4., qkv_bias=True,
+                              norm_layer=partial(nn.LayerNorm, eps=1e-6), use_dense_prediction=use_dense_prediction,
+                              **spec)
     hk = head_kwargs or {}
     net.head = DINOHead(net.num_features, out_dim, norm_last_layer=norm_last_layer, **hk)
     if use_dense_prediction:
@@ -229,7 +242,7 @@ def make_step(arch: str = "swin_tiny_w7", out_dim: int = 65536, ncrops: int = 10
               teacher_temp: float = 0.04, seed: int = 0, optimizer: str = "fused", cuda_graph: bool = False):
     """Build student/teacher/loss/optimizer the way train_esvit does (main_esvit.py:235-435) and return
     (step, student, teacher, loss)."""
-    spec = dict(spec if spec is not None else SWIN_SPECS[arch])
+    spec = dict(spec if spec is not None else (VIT_SPECS[arch] if arch in VIT_SPECS else SWIN_SPECS[arch]))
     if drop_path is not None:
         spec["drop_path_rate"] = drop_path
     torch.manual_seed(seed)

@@ -579,6 +579,150 @@ class TokenMeanGroupsFn(Function):
         return d, None
 
 
+class MhsaGroupsFn(Function):
+    """Whole-sequence multi-head attention at head dim 64 (models/vision_transformer.py:83-95) over several resolution
+    groups stored back to back: qkv bf16 [T, 3C] (qkv GEMM output incl. bias), group g = (B, L, row0) = rows
+    [row0, row0 + B*L) holding B sequences of L tokens -> bf16 [T, C].  One launch per group on pointer offsets.
+    qkv_bias (fp32 [3C]) only receives its gradient: the fixed-order column sums of dqkv (esvit_colsum)."""
+
+    @staticmethod
+    def forward(ctx, qkv, qkv_bias, groups, num_heads: int, scale: float):
+        qkv = _chk(qkv, BF16, "qkv")
+        T, C3 = qkv.shape
+        C = C3 // 3
+        if sum(B * L for B, L, _ in groups) != T:
+            raise ValueError(f"groups {groups} do not cover the {T} rows of qkv")
+        out = torch.empty(T, C, dtype=BF16, device=qkv.device)
+        lse = torch.empty(T * num_heads, dtype=F32, device=qkv.device)  # per group [B, nH, L] at row0 * nH
+        for B, L, r0 in groups:
+            _lib.call("esvit_mhsa_fwd", _po(qkv, r0 * C3), _po(out, r0 * C), _po(lse, r0 * num_heads), B, L, C, num_heads,
+                      scale, _stream())
+        ctx.save_for_backward(qkv, out, lse)
+        ctx.meta = (tuple(groups), num_heads, scale, qkv_bias is not None)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        qkv, out, lse = ctx.saved_tensors
+        groups, nH, scale, has_bias = ctx.meta
+        g = _chk(g, BF16, "g")
+        T, C3 = qkv.shape
+        C = C3 // 3
+        dqkv = torch.empty_like(qkv)
+        dvec = torch.empty_like(lse)
+        for B, L, r0 in groups:
+            _lib.call("esvit_mhsa_bwd", _po(qkv, r0 * C3), _po(out, r0 * C), _po(g, r0 * C), _po(lse, r0 * nH),
+                      _po(dvec, r0 * nH), _po(dqkv, r0 * C3), B, L, C, nH, scale, _stream())
+        return dqkv, (colsum(dqkv) if has_bias else None), None, None, None
+
+
+def mhsa(qkv: Tensor, num_heads: int, scale: float) -> Tuple[Tensor, Tensor]:
+    """(out bf16 [B*L, C], lse fp32 [B, nH, L]) of MhsaGroupsFn's kernel on qkv bf16 [B, L, 3C]; not differentiable."""
+    qkv = _chk(qkv, BF16, "qkv")
+    B, L, C3 = qkv.shape
+    out = torch.empty(B * L, C3 // 3, dtype=BF16, device=qkv.device)
+    lse = torch.empty(B, num_heads, L, dtype=F32, device=qkv.device)
+    _lib.call("esvit_mhsa_fwd", _p(qkv), _p(out), _p(lse), B, L, C3 // 3, num_heads, scale, _stream())
+    return out, lse
+
+
+def vit_patches(imgs: Sequence[Tensor], p: int) -> Tensor:
+    """fp32 [B_g, 3, S_g, S_g] crops -> the bf16 patch rows [sum_g B_g N_g, 3p^2] of all of them, back to back, in the
+    conv weight's (c, ky, kx) flatten order (the input of the patch-projection GEMM)."""
+    imgs = [_chk(im, F32, "img") for im in imgs]
+    rows = [im.shape[0] * (im.shape[2] // p) * (im.shape[3] // p) for im in imgs]
+    out = torch.empty(sum(rows), 3 * p * p, dtype=BF16, device=imgs[0].device)
+    r0 = 0
+    for im, n in zip(imgs, rows):
+        B, Cin, H, W = im.shape
+        if Cin != 3 or H != W or H % p != 0:
+            raise ValueError(f"expected square crops [B, 3, S, S] with S a multiple of {p}, got {tuple(im.shape)}")
+        _lib.call("esvit_vit_patches", _p(im), _po(out, r0 * 3 * p * p), B, H, p, _stream())
+        r0 += n
+    return out
+
+
+class VitTokensGroupsFn(Function):
+    """The ViT residual stream of several resolution groups, back to back in ONE fp32 tensor [sum_g B_g (1+N_g), D]:
+    sequence b of group g = cat(cls_token, pe[b]) + pos_g (models/vision_transformer.py:237-240).
+    pe bf16 [sum_g B_g N_g, D] is the patch-projection GEMM output (bias included); groups = ((B, N), ...);
+    pos: one fp32 [1, 1+N_g, D] tensor per group.  bias (fp32 [D]) only receives its gradient (column sums of the patch
+    rows' gradient)."""
+
+    @staticmethod
+    def forward(ctx, pe, bias, cls_token, groups, *pos):
+        pe, cls = _chk(pe, BF16, "pe"), _chk(cls_token, F32, "cls_token")
+        pos = [_chk(q, F32, "pos_embed") for q in pos]
+        D = pe.shape[-1]
+        T = sum(B * (N + 1) for B, N in groups)
+        x = torch.empty(T, D, dtype=F32, device=pe.device)
+        p0 = x0 = 0
+        for (B, N), q in zip(groups, pos):
+            if q.numel() != (N + 1) * D:
+                raise ValueError(f"pos_embed of {q.numel()} values for {N} patches of width {D}")
+            _lib.call("esvit_vit_tokens_fwd", _po(pe, p0 * D), _p(cls), _p(q), _po(x, x0 * D), B, N, D, _stream())
+            p0 += B * N
+            x0 += B * (N + 1)
+        ctx.meta = (tuple(groups), D, pe.shape[0], tuple(tuple(q.shape) for q in pos))
+        return x
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        groups, D, npe, pos_shapes = ctx.meta
+        g = _chk(g, F32, "g")
+        dpe = torch.empty(npe, D, dtype=BF16, device=g.device)
+        dbias = torch.empty(D, dtype=F32, device=g.device)
+        dcls = torch.empty(1, 1, D, dtype=F32, device=g.device)
+        dpos, p0, x0 = [], 0, 0
+        for gi, ((B, N), shp) in enumerate(zip(groups, pos_shapes)):
+            d = torch.empty(shp, dtype=F32, device=g.device)
+            _lib.call("esvit_vit_tokens_bwd", _po(g, x0 * D), _po(dpe, p0 * D), _p(d), _p(dbias), _p(dcls),
+                      1 if gi else 0, B, N, D, _stream())
+            dpos.append(d)
+            p0 += B * N
+            x0 += B * (N + 1)
+        return (dpe, dbias, dcls, None) + tuple(dpos)
+
+
+class VitSplitGroupsFn(Function):
+    """x fp32 [sum_g B_g (1+N_g), D] (the final norm's output) -> (cls rows [sum_g B_g, D], region rows
+    [sum_g B_g N_g, D]), group-major then image-major as the reference concatenates them; groups = ((B, N), ...)."""
+
+    @staticmethod
+    def forward(ctx, x, groups):
+        x = _chk(x, F32, "x")
+        D = x.shape[-1]
+        nb = sum(B for B, _ in groups)
+        cls = torch.empty(nb, D, dtype=F32, device=x.device)
+        region = torch.empty(sum(B * N for B, N in groups), D, dtype=F32, device=x.device)
+        _vit_split(x, cls, region, groups, 0)
+        ctx.meta = (tuple(groups), tuple(x.shape))
+        return cls, region
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_cls, g_region):
+        groups, shape = ctx.meta
+        g_cls = _chk(g_cls, F32, "g_cls")
+        g_region = _chk(g_region, F32, "g_region")
+        dx = torch.empty(shape, dtype=F32, device=(g_cls if g_cls is not None else g_region).device)
+        _vit_split(dx, g_cls, g_region, groups, 1)
+        return dx, None
+
+
+def _vit_split(x, cls, region, groups, direction):
+    D = x.shape[-1]
+    x0 = b0 = q0 = 0
+    for B, N in groups:
+        _lib.call("esvit_vit_split", _po(x, x0 * D), _po(cls, b0 * D) if cls is not None else None,
+                  _po(region, q0 * D) if region is not None else None, B, N, D, direction, _stream())
+        x0 += B * (N + 1)
+        b0 += B
+        q0 += B * N
+
+
 @torch.no_grad()
 def window_attention_probs(qkv: Tensor, qkv_bias: Tensor, bias_table: Tensor, H: int, W: int, num_heads: int, ws: int,
                            shift: int, scale: float, bias_exp: Optional[Tensor] = None) -> Tensor:

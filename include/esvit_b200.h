@@ -177,10 +177,32 @@ int esvit_center_ema(const float* center, const float* colsum, float rows_total,
  * region_match: for every student region token of every crop v != iq, the FIRST arg-max over the Tg teacher tokens
  * of view iq (same image) of the cosine similarity.  sn fp32 [Rs,P] rows ordered (crop, image, token) with 2 global
  * crops of Tg tokens then ncrops-2 local crops of Tl tokens; tn fp32 [2*B*Tg, P].
- * idx_out int64 [2, ncrops, B, Tg] (slots of v == iq or i >= T_v untouched); trow int32 [Rs,2] teacher region rows. */
+ * idx_out int64 [2, ncrops, B, Tg] (slots of v == iq or i >= T_v untouched); trow int32 [Rs,2] teacher region rows.
+ * Teacher rows that do not fit shared memory at once (Tg*P*4 > 220 KB, ViT) are streamed in chunks; same indices. */
 int esvit_normalize_rows(const float* x, float* y, long long R, int P, float eps, void* stream);
 int esvit_region_match(const float* sn, const float* tn, int B, int ncrops, int Tg, int Tl, int P,
                        long long* idx_out, int* trow, void* stream);
+
+/* ---- ViT whole-sequence attention, head dim 64 ------------------------ models/vision_transformer.py:83-95
+ * qkv bf16 [B*L, 3C] (qkv GEMM output incl. bias; channels [q|k|v][head][64]), C = nH*64 (else ESVIT_ERR_BAD_ARG),
+ * out bf16 [B*L, C] in (attn @ v).transpose(1, 2).reshape(B, L, C) order, lse fp32 [B, nH, L] (natural log).
+ * bwd: dout bf16 [B*L, C]; dvec fp32 [B*nH*L] workspace; dqkv bf16 [B*L, 3C] fully written (no atomics). */
+int esvit_mhsa_fwd(const void* qkv, void* out, float* lse, int B, int L, int C, int nH, float scale, void* stream);
+int esvit_mhsa_bwd(const void* qkv, const void* out, const void* dout, const float* lse, float* dvec, void* dqkv,
+                   int B, int L, int C, int nH, float scale, void* stream);
+
+/* ---- ViT token embedding ------------------------------------------ models/vision_transformer.py:124-139, 233-251
+ * patches: img fp32 [B,3,S,S] -> bf16 [B*N, 3p^2], N = (S/p)^2, columns in the conv weight's (c, ky, kx) order (p even).
+ * tokens_fwd: x fp32 [B, 1+N, D] = cat(cls, pe bf16 [B*N, D]) + pos fp32 [1+N, D].
+ * tokens_bwd: g fp32 [B, 1+N, D] -> dpe bf16 [B*N, D], dpos fp32 [1+N, D] (written); dbias, dcls fp32 [D] written
+ *   (accumulate = 0) or added to (accumulate = 1).  Fixed summation order, no atomics.
+ * split: dir 0: x fp32 [B, 1+N, D] -> cls [B, D], region [B*N, D]; dir 1: gradients of cls / region (either may be
+ *   null = zero) -> x. */
+int esvit_vit_patches(const float* img, void* patches, int B, int S, int p, void* stream);
+int esvit_vit_tokens_fwd(const void* pe, const float* cls, const float* pos, float* x, int B, int N, int D, void* stream);
+int esvit_vit_tokens_bwd(const float* g, void* dpe, float* dpos, float* dbias, float* dcls, int accumulate, int B, int N,
+                         int D, void* stream);
+int esvit_vit_split(float* x, float* cls, float* region, int B, int N, int D, int dir, void* stream);
 
 /* ---- optimiser-side multi-tensor kernels (host arrays of device pointers) ----------------------------------
  * ema_multi: teacher = teacher*m + student*(1-m), bit-exact with main_esvit.py:587-590.
