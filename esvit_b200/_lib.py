@@ -71,6 +71,9 @@ SIGNATURES = {
     "esvit_knn_prep": [P, P, P, P, L, L, I, P],
     "esvit_knn_select": [P, L, P, P, P, P, P, I, I, I, I, I, P, P, P, P, P, P],
     "esvit_knn_vote": [P, P, P, P, L, I, F, I, P, P],
+    "esvit_augment_coeffs": [P, P, P, I, I, P],
+    "esvit_augment_resize_h": [P, P, P, P, P, I, L, P],
+    "esvit_augment_color": [P, P, P, P, P, I, I, I, P],
 }
 
 _lib = None

@@ -244,6 +244,23 @@ int esvit_knn_select(const void* S, long long ld, const float* a, const float* b
 int esvit_knn_vote(const float* sims, const long long* idx, const long long* train_labels, const long long* test_labels,
                    long long M, int k, float T, int num_classes, long long* hits, void* stream);
 
+/* ---- multi-crop augmentation (DataAugmentationDINO) on decoded uint8 images ---------------- datasets/build.py:203-261
+ * Pillow's arithmetic for RandomResizedCrop(bicubic) / hflip / ColorJitter / RandomGrayscale / ImageFilter.GaussianBlur /
+ * ImageOps.solarize, then ToTensor + Normalize, for every crop of a batch (esvit_b200/augment.py builds the arguments).
+ * params fp64 [ncrops, 18] (augment.PARAM_FIELDS); meta int64 [ncrops, 9]: source byte offset into src (uint8 HWC), source
+ * H, W, output size S, byte offset into tmp (uint8 [h, S, 3] per crop), int32 offset into coef (S * (4 + kh + kv) per
+ * crop), horizontal / vertical tap counts kh = 2 ceil(2 max(1, w / S)) + 1 and kv (same with h), fp32 output address of
+ * the crop's [3, S, S].  Every offset is 64-bit.
+ * coeffs: both axes' bounds and 22-bit fixed-point bicubic coefficients of every crop into coef; max_S = max S.
+ * resize_h: the horizontal pass of every box row (flip applied) into tmp; max_pixels = max over crops of h * S.
+ * color: crops [crop0, crop0 + ncrops), all of output size S <= 241: vertical pass, colour ops, blur, solarize, normalize
+ *   with norm fp32 [6] = (mean[3], std[3]); the fp32 crop is written with streaming stores. */
+int esvit_augment_coeffs(const double* params, const long long* meta, int* coef, int ncrops, int max_S, void* stream);
+int esvit_augment_resize_h(const unsigned char* src, const double* params, const long long* meta, const int* coef,
+                           unsigned char* tmp, int ncrops, long long max_pixels, void* stream);
+int esvit_augment_color(const double* params, const long long* meta, const int* coef, const unsigned char* tmp,
+                        const float* norm, int crop0, int ncrops, int S, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
