@@ -37,6 +37,7 @@ SIGNATURES = {
     "esvit_gemm_mul_colsum2": [P, P, P, P, P, P, L, I, I, I, I, P],
     "esvit_gemm_wgrad_ws_floats": [I, I],
     "esvit_gemm_wgrad": [P, P, P, P, L, I, I, I, I, P],
+    "esvit_mlp_fwd": [P, P, P, P, P, P, P, P, L, I, P],
     "esvit_gelu_fwd": [P, P, L, P],
     "esvit_gelu_bwd": [P, P, P, L, P],
     "esvit_gelu_bwd_dbias": [P, P, P, P, L, I, P],
@@ -138,6 +139,7 @@ _META = {
                                   "pre": a[4] is not None and a[4].value is not None},
     "esvit_gemm_mul_colsum2": lambda a: {"M": int(a[6]), "N": int(a[7]), "K": int(a[8])},
     "esvit_gemm_wgrad": lambda a: {"T": int(a[4]), "N": int(a[5]), "K": int(a[6])},
+    "esvit_mlp_fwd": lambda a: {"M": int(a[8]), "C": int(a[9]), "student": a[6] is not None and a[6].value is not None},
     "esvit_add_ln_fwd": lambda a: {"T": int(a[-3]), "C": int(a[-2]), "has_x": a[0] is not None and a[0].value is not None,
                                    "has_delta": a[1] is not None and a[1].value is not None},
     "esvit_add_ln_bwd": lambda a: {"T": int(a[-3]), "C": int(a[-2])},

@@ -145,6 +145,50 @@ __device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t da, uint64_
       : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
 }
 
+// D[64 x 64] (+)= A[64 x 16] . B[16 x 64], both K-major from shared memory
+__device__ __forceinline__ void wgmma_ss_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+// D[64 x N] (+)= A[64 x 16] . B[16 x N]: A from registers (the m64k16 fragment, four bf16 pairs per thread), B K-major
+// from shared memory; N = 2 * size of d (the back-to-back MLP's fc2 at N = C)
+__device__ __forceinline__ void wgmma_rs(float (&d)[48], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %53, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, "
+      "{%48, %49, %50, %51}, %52, p, 1, 1, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "{%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_rs(float (&d)[96], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %101, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n192k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, "
+      "{%96, %97, %98, %99}, %100, p, 1, 1, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+
 template <int BN, int TA, int TB>
 __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
   if constexpr (BN == 256) wgmma_n256<TA, TB>(d, da, db, scale_d);
@@ -484,6 +528,232 @@ __global__ void __launch_bounds__(128 * (WG + 1), 1) gemm_kernel(const __grid_co
   }
 }
 
+// ---- back-to-back MLP forward: y = GELU(x . W1^T + b1) . W2^T + b2, the hidden activation never re-read from HBM ------
+// x [M, C], W1 [4C, C], W2 [C, 4C] bf16.  Persistent over 128-row items; the producer TMA-loads an item's x tile once
+// (double buffered across items) and streams the weights through the ring in chunks of 64 hidden units (W1 rows j*64..,
+// W2 columns j*64..).  Each consumer warpgroup owns 64 rows and, per chunk in ascending order:
+//   acc1 = x . W1_chunk^T          C/16 k16 steps of wgmma m64n64k16 (both operands from shared memory)
+//   h    = GELU(acc1 + b1)         the gemm_kernel EPI_GELU arithmetic, packed to bf16: the m64n64 accumulator fragment
+//                                  of 8-column blocks 2s, 2s + 1 IS the m64k16 A-register fragment of k16 step s
+//   acc2 += h . W2_chunk^T         4 k16 steps of wgmma m64nCk16 with A from registers
+// so fc1 runs the same k16 sequence as gemm_kernel over K = C and fc2 the same k16 sequence over K = 4C as its BK = 64
+// mainloop: y, h and gelu' equal the two-launch chain's.  With STORE (the student) h and gelu' of each chunk leave
+// through the bf16 staging path for the backward; y = acc2 + b2 leaves the same way at the end of the item.  acc2 [64 x C]
+// lives in registers for the whole item, which bounds C: C = 256 fits neither the registers nor (with a double-buffered
+// x tile) the shared memory.
+template <int C>
+struct MlpCfg {
+  static constexpr int BM = 128, HB = 64;               // rows per item, hidden units per chunk
+  static constexpr int KB = (C + 63) / 64;              // 64-column TMA boxes across C (the last zero-filled past C)
+  static constexpr int NH = 4 * C / HB;                 // hidden chunks per item
+  static constexpr int X_BYTES = KB * BM * 128;         // x tile: KB boxes of [128 rows][128 B]
+  static constexpr int W1_BYTES = KB * HB * 128;        // W1 chunk: KB boxes of [64 hidden rows][128 B]
+  static constexpr int W2_BYTES = C * 128;              // W2 chunk: one box of [C rows][64 hidden = 128 B]
+  static constexpr int STAGE_BYTES = W1_BYTES + W2_BYTES;
+  static constexpr int CHUNK_BYTES = BM * 128;          // one [128 rows x 64 columns] bf16 output chunk, 128B-swizzled
+  static constexpr int EP_BYTES = 2 * CHUNK_BYTES;      // (h, gelu') of a hidden chunk; y chunks alternate over both
+  static constexpr int BAR_BYTES = 128;
+  static constexpr int STAGES_RAW = (SMEM_LIMIT - 1024 - BAR_BYTES - 2 * X_BYTES - EP_BYTES) / STAGE_BYTES;
+  static constexpr int STAGES = STAGES_RAW > 4 ? 4 : STAGES_RAW;
+  static constexpr int SMEM = 1024 + 2 * X_BYTES + STAGES * STAGE_BYTES + EP_BYTES + BAR_BYTES;
+  static_assert(C % 32 == 0 && C <= 192, "acc2 [64 x C] must fit the consumer registers; C / 8 even");
+  static_assert(STAGES >= 2, "weight ring too shallow");
+  static_assert(SMEM <= SMEM_LIMIT, "shared memory budget");
+  static_assert((2 * STAGES + 4) * 8 <= BAR_BYTES, "mbarrier area");
+};
+
+struct MlpParams {
+  const float* b1;  // [4C] or nullptr
+  const float* b2;  // [C] or nullptr
+  int M;
+};
+
+// map_x: x box [64 cols][128 rows]; map_w1: [64 cols][64 rows]; map_w2: [64 cols][C rows]; map_y / map_h / map_g: output
+// boxes [64 cols][64 rows] (map_h / map_g unused without STORE)
+template <int C, bool STORE>
+__global__ void __launch_bounds__(384, 1) mlp_fwd_kernel(const __grid_constant__ CUtensorMap map_x,
+                                                         const __grid_constant__ CUtensorMap map_w1,
+                                                         const __grid_constant__ CUtensorMap map_w2,
+                                                         const __grid_constant__ CUtensorMap map_y,
+                                                         const __grid_constant__ CUtensorMap map_h,
+                                                         const __grid_constant__ CUtensorMap map_g, const MlpParams p) {
+  using G = MlpCfg<C>;
+  constexpr int BM = G::BM, KB = G::KB, NH = G::NH, STAGES = G::STAGES;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  // x[2] | [STAGES][W1 | W2] | (h, gelu') staging | mbarriers; every tile 1024-byte aligned in the shared address space
+  uint8_t* xs = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* ws = xs + 2 * G::X_BYTES;
+  uint8_t* ep = ws + STAGES * G::STAGE_BYTES;
+  uint64_t* full = reinterpret_cast<uint64_t*>(ep + G::EP_BYTES);
+  uint64_t* empty = full + STAGES;
+  uint64_t* x_full = empty + STAGES;
+  uint64_t* x_empty = x_full + 2;
+
+  const int wg = threadIdx.x >> 7;
+  const int num_items = (p.M + BM - 1) / BM;
+  if (threadIdx.x == 0) {
+    asm volatile("prefetch.tensormap [%0];\n" ::"l"(&map_x) : "memory");
+    asm volatile("prefetch.tensormap [%0];\n" ::"l"(&map_w1) : "memory");
+    asm volatile("prefetch.tensormap [%0];\n" ::"l"(&map_w2) : "memory");
+    for (int i = 0; i < STAGES; i++) { mbar_init(&full[i], 1); mbar_init(&empty[i], 256); }
+    for (int i = 0; i < 2; i++) { mbar_init(&x_full[i], 1); mbar_init(&x_empty[i], 256); }
+    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+  }
+  __syncthreads();
+
+  if (wg == 2) {
+    // ===================== TMA producer: one thread of the last warpgroup =====================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+    if (threadIdx.x == 256) {
+      int stage = 0;
+      uint32_t phase = 0;
+      int local = 0;
+      for (int item = blockIdx.x; item < num_items; item += gridDim.x, local++) {
+        const int m0 = item * BM, xb = local & 1;
+        // x buffer xb was last read by the fc1 of item local - 2
+        mbar_wait(&x_empty[xb], ((local >> 1) & 1) ^ 1);
+        mbar_expect_tx(&x_full[xb], G::X_BYTES);
+#pragma unroll
+        for (int kb = 0; kb < KB; kb++)
+          tma_load_2d(smem_u32(xs + xb * G::X_BYTES + kb * BM * 128), &map_x, &x_full[xb], kb * 64, m0);
+        for (int j = 0; j < NH; j++) {
+          mbar_wait(&empty[stage], phase ^ 1);
+          const uint32_t sw = smem_u32(ws + stage * G::STAGE_BYTES);
+          mbar_expect_tx(&full[stage], G::STAGE_BYTES);
+#pragma unroll
+          for (int kb = 0; kb < KB; kb++) tma_load_2d(sw + kb * 8192, &map_w1, &full[stage], kb * 64, j * 64);
+          tma_load_2d(sw + G::W1_BYTES, &map_w2, &full[stage], j * 64, 0);
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    // ===================== consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of the item =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+    const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
+    const int frag_col = 2 * (lane & 3);
+    const uint32_t lrow = (uint32_t)(warp * 16 + (lane & 15)) * 128u, lsw = lane & 7, lblk = lane >> 4;
+    const bool leader = t == 0;   // issues this warpgroup's stores and waits for them
+    const uint32_t hbuf = smem_u32(ep) + wg * 8192;   // this warpgroup's rows of the h staging chunk (+ CHUNK_BYTES: gelu')
+    int stage = 0;
+    uint32_t phase = 0;
+    int local = 0;
+    for (int item = blockIdx.x; item < num_items; item += gridDim.x, local++) {
+      const int m0 = item * BM, xb = local & 1;
+      const uint64_t da = make_smem_desc(smem_u32(xs + xb * G::X_BYTES) + wg * 8192, false);   // this warpgroup's 64 rows
+      float acc1[32], acc2[C / 2];
+      mbar_wait(&x_full[xb], (local >> 1) & 1);
+      for (int j = 0; j < NH; j++) {
+        // fc1: acc1 = x . W1_chunk^T
+        {
+          const uint64_t db = make_smem_desc(smem_u32(ws + stage * G::STAGE_BYTES), false);
+          mbar_wait(&full[stage], phase);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < C / 16; k++)   // descriptor units of 16 B: k16 step = 32 B, x box = BM * 128 B, W1 box = 8 KB
+            wgmma_ss_n64(acc1, da + (k >> 2) * (BM * 128 >> 4) + (k & 3) * 2, db + (k >> 2) * (8192 >> 4) + (k & 3) * 2,
+                         k ? 1u : 0u);
+          wgmma_commit();
+        }
+        wgmma_wait<0>();   // fc1 of chunk j has retired
+        if (j == NH - 1) mbar_arrive(&x_empty[xb]);   // the item's last fc1 has read x
+        if constexpr (STORE) {
+          // the previous chunk's stores have read the staging buffers before they are overwritten
+          if (leader) bulk_wait_read<0>();
+          named_barrier(1 + wg, 128);
+        }
+        // bias + GELU (+ gelu' to the staging buffer) -> bf16 A fragments of the 4 k16 steps of fc2
+        uint32_t af[4][4];
+#pragma unroll
+        for (int s = 0; s < 4; s++) {
+          const float* a0 = acc1 + 8 * s;   // 8-column blocks 2s, 2s + 1 of the chunk
+          float b[4] = {0.f, 0.f, 0.f, 0.f};
+          if (p.b1) {
+#pragma unroll
+            for (int u = 0; u < 2; u++) {
+              const float2 bb = __ldg(reinterpret_cast<const float2*>(p.b1 + j * 64 + (2 * s + u) * 8 + frag_col));
+              b[2 * u] = bb.x; b[2 * u + 1] = bb.y;
+            }
+          }
+          uint32_t d[4];
+#pragma unroll
+          for (int q = 0; q < 4; q++) {
+            const float v0 = a0[2 * q] + b[2 * (q >> 1)], v1 = a0[2 * q + 1] + b[2 * (q >> 1) + 1];
+            if constexpr (STORE) {
+              float d0, d1;
+              const float y0 = gelu_fwd_grad(v0, d0), y1 = gelu_fwd_grad(v1, d1);
+              af[s][q] = pack_bf162(y0, y1);
+              d[q] = pack_bf162(d0, d1);
+            } else {
+              af[s][q] = pack_bf162(gelu_fwd(v0), gelu_fwd(v1));
+            }
+          }
+          if constexpr (STORE) {
+            const uint32_t addr = hbuf + lrow + (((2 * s + lblk) ^ lsw) << 4);
+            stmatrix_x4(addr, af[s][0], af[s][1], af[s][2], af[s][3]);
+            stmatrix_x4(addr + G::CHUNK_BYTES, d[0], d[1], d[2], d[3]);
+          }
+        }
+        if constexpr (STORE) fence_proxy_async();
+        // fc2: acc2 += h_chunk . W2_chunk^T.  It retires before the next fc1 is issued, so acc1 and the A fragments are
+        // never live at once: at C = 192 acc2 (96) + acc1 (32) + the fragments (16) would not fit next to the addressing.
+        const uint64_t d2 = make_smem_desc(smem_u32(ws + stage * G::STAGE_BYTES) + G::W1_BYTES, false);
+        wgmma_fence();
+#pragma unroll
+        for (int s = 0; s < 4; s++) wgmma_rs(acc2, af[s], d2 + s * 2, (j > 0 || s > 0) ? 1u : 0u);
+        wgmma_commit();
+        if constexpr (STORE) {
+          named_barrier(1 + wg, 128);
+          if (leader) {
+            const int gr = m0 + 64 * wg;
+            if (gr < p.M) {
+              tma_store_2d(&map_h, hbuf, j * 64, gr);
+              tma_store_2d(&map_g, hbuf + G::CHUNK_BYTES, j * 64, gr);
+            }
+            bulk_commit();
+          }
+        }
+        wgmma_wait<0>();   // fc2 of chunk j has retired: its stage is free
+        mbar_arrive(&empty[stage]);
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      // ---- y = acc2 + b2: 64-column chunks alternating over the two staging buffers (the gemm_kernel EPI_BIAS path)
+#pragma unroll
+      for (int c = 0; c < KB; c++) {
+        const uint32_t buf = smem_u32(ep + (c & 1) * G::CHUNK_BYTES) + wg * 8192;
+        if (leader) bulk_wait_read<0>();
+        named_barrier(1 + wg, 128);
+#pragma unroll
+        for (int jj = 0; jj < 8; jj += 2) {
+          const int i = c * 8 + jj;   // 8-column blocks i, i + 1 of y
+          if (i >= C / 8) continue;
+          const float* a0 = acc2 + 4 * i;
+          float b[4] = {0.f, 0.f, 0.f, 0.f};
+          if (p.b2) {
+#pragma unroll
+            for (int u = 0; u < 2; u++) {
+              const float2 bb = __ldg(reinterpret_cast<const float2*>(p.b2 + (i + u) * 8 + frag_col));
+              b[2 * u] = bb.x; b[2 * u + 1] = bb.y;
+            }
+          }
+          uint32_t o[4];
+#pragma unroll
+          for (int q = 0; q < 4; q++) o[q] = pack_bf162(a0[2 * q] + b[2 * (q >> 1)], a0[2 * q + 1] + b[2 * (q >> 1) + 1]);
+          stmatrix_x4(buf + lrow + (((jj + lblk) ^ lsw) << 4), o[0], o[1], o[2], o[3]);
+        }
+        fence_proxy_async();
+        named_barrier(1 + wg, 128);
+        if (leader) {
+          const int gr = m0 + 64 * wg;
+          if (gr < p.M) tma_store_2d(&map_y, buf, c * 64, gr);
+          bulk_commit();
+        }
+      }
+    }
+    if (t == 0) bulk_wait_all();   // the CTA's last stores have completed before it exits
+  }
+}
+
 // ------------------------------------------------------------------------------------------------------------------
 typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                              const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -512,6 +782,38 @@ static bool make_map(CUtensorMap* map, const void* ptr, long long rows, long lon
   return enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+template <int C, bool STORE>
+static int mlp_launch(const void* x, const void* w1, const float* b1, const void* w2, const float* b2, void* y, void* h,
+                      void* g, int M, void* stream) {
+  using G = MlpCfg<C>;
+  CUtensorMap mx, m1, m2, my, mh = {}, mg = {};
+  if (!make_map(&mx, x, M, C, G::BM) || !make_map(&m1, w1, 4 * C, C, 64) || !make_map(&m2, w2, C, 4 * C, C) ||
+      !make_map(&my, y, M, C, 64))
+    return ESVIT_ERR_BAD_ARG;
+  if (STORE && (!make_map(&mh, h, M, 4 * C, 64) || !make_map(&mg, g, M, 4 * C, 64))) return ESVIT_ERR_BAD_ARG;
+  auto kernel = mlp_fwd_kernel<C, STORE>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, G::SMEM);
+    if (e != cudaSuccess) return (int)e;
+    attr_set = true;
+  }
+  const int items = (M + G::BM - 1) / G::BM;
+  int grid = esvit_num_sms();
+  if (grid > items) grid = items;
+  MlpParams p;
+  p.b1 = b1; p.b2 = b2; p.M = M;
+  kernel<<<grid, 384, G::SMEM, (cudaStream_t)stream>>>(mx, m1, m2, my, mh, mg, p);
+  return (int)cudaGetLastError();
+}
+
+template <int C>
+static int mlp_launch_c(const void* x, const void* w1, const float* b1, const void* w2, const float* b2, void* y, void* h,
+                        void* g, int M, void* stream) {
+  return h ? mlp_launch<C, true>(x, w1, b1, w2, b2, y, h, g, M, stream)
+           : mlp_launch<C, false>(x, w1, b1, w2, b2, y, h, g, M, stream);
 }
 
 // colsum[n] += sum over the CTAs' private rows
@@ -722,6 +1024,25 @@ ESVIT_API int esvit_gemm_wgrad(const void* dy, const void* x, float* dw, float* 
   const long long n4 = (long long)N * K / 4;
   hg::split_fold_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(ws, splits, n4, dw, accumulate);
   ESVIT_LAUNCH_CHECK();
+}
+
+// y[M,C] (bf16) = GELU(x[M,C] . w1[4C,C]^T + b1) . w2[C,4C]^T + b2 in one kernel (hg::mlp_fwd_kernel): bit-identical to
+// esvit_gemm_bf16 act 1 followed by esvit_gemm_bf16 act 0.  h, gelu_grad [M,4C] bf16: both NULL (no-grad forward), or both
+// set to receive GELU(pre-activation) and gelu'(pre-activation) for the backward.  C in {96, 128, 192}; biases fp32 or NULL;
+// every matrix 16-byte aligned.
+ESVIT_API int esvit_mlp_fwd(const void* x, const void* w1, const float* b1, const void* w2, const float* b2, void* y,
+                            void* h, void* gelu_grad, long long M, int C, void* stream) {
+  auto aligned = [](const void* q, uintptr_t a) { return ((uintptr_t)q & (a - 1)) == 0; };
+  if (M <= 0 || M > 0x7fffffffLL || !x || !w1 || !w2 || !y || (h == nullptr) != (gelu_grad == nullptr)) return ESVIT_ERR_BAD_ARG;
+  if (!aligned(x, 16) || !aligned(w1, 16) || !aligned(w2, 16) || !aligned(y, 16) || !aligned(h, 16) ||
+      !aligned(gelu_grad, 16) || !aligned(b1, 8) || !aligned(b2, 8))
+    return ESVIT_ERR_BAD_ARG;
+  switch (C) {
+    case 96: return hg::mlp_launch_c<96>(x, w1, b1, w2, b2, y, h, gelu_grad, (int)M, stream);
+    case 128: return hg::mlp_launch_c<128>(x, w1, b1, w2, b2, y, h, gelu_grad, (int)M, stream);
+    case 192: return hg::mlp_launch_c<192>(x, w1, b1, w2, b2, y, h, gelu_grad, (int)M, stream);
+  }
+  return ESVIT_ERR_BAD_ARG;
 }
 
 // ---- first-generation entry points, served by the same kernel family ------------------------------------------------

@@ -67,18 +67,27 @@ class LinearFn(Function):
 
 
 class MlpFn(Function):
-    """fc2(gelu(fc1(x))) (models/swin_transformer.py:31-35).  forward: h, gelu' from ONE GEMM (bias + exact GELU epilogue),
-    y = h . W2^T + b2.  backward: d(pre) = (dy . W2) * gelu' with the fc1 bias gradient as column sums, all in one GEMM
-    epilogue; dx = d(pre) . W1; dW1, dW2 in fp32.  b2's gradient is produced by the consumer (residual add + LN backward)."""
+    """fc2(gelu(fc1(x))) (models/swin_transformer.py:31-35).  forward at C in ops.MLP_FUSED_C (Swin stages 0-1): ONE
+    back-to-back kernel (esvit_mlp_fwd) writes y and, when a gradient is needed, h and gelu'; at other C: h, gelu' from ONE
+    GEMM (bias + exact GELU epilogue), y = h . W2^T + b2.  backward: d(pre) = (dy . W2) * gelu' with the fc1 bias gradient
+    as column sums, all in one GEMM epilogue; dx = d(pre) . W1; dW1, dW2 in fp32.  b2's gradient is produced by the consumer (residual add + LN backward)."""
 
     @staticmethod
     def forward(ctx, x, w1p, w1, b1, w2p, w2, b2):
         need = any(ctx.needs_input_grad)  # (grad mode is always off inside Function.forward: needs_input_grad is the signal)
-        if need:
-            h, pre = ops.gemm(x, w1, b1, act=1, want_pre=True)
+        C = x.shape[-1]
+        if C in ops.MLP_FUSED_C and w1.shape[0] == 4 * C:
+            # one back-to-back kernel: h goes to HBM only when the backward needs it, and is never read back here
+            if need:
+                y, h, pre = ops.mlp_fwd(x, w1, b1, w2, b2, want_h=True)
+            else:
+                y, h, pre = ops.mlp_fwd(x, w1, b1, w2, b2), None, None
         else:
-            h, pre = ops.gemm(x, w1, b1, act=1), None
-        y = ops.gemm(h, w2, b2)
+            if need:
+                h, pre = ops.gemm(x, w1, b1, act=1, want_pre=True)
+            else:
+                h, pre = ops.gemm(x, w1, b1, act=1), None
+            y = ops.gemm(h, w2, b2)
         ctx.save_for_backward(x, w1, w2, pre, h)
         ctx.keys = (("w", w1p.data_ptr()), tuple(w1p.shape), ("w", w2p.data_ptr()), tuple(w2p.shape))
         ctx.bias_meta = (b1.shape, b1.device, b1.data_ptr())

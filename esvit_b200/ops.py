@@ -855,6 +855,24 @@ def gemm_mul_colsum(a: Tensor, b: Tensor, mult: Tensor, colsum: Tensor, b_mn: bo
     return out
 
 
+MLP_FUSED_C = (96, 128, 192)  # include/esvit_b200.h: the widths esvit_mlp_fwd serves
+
+
+def mlp_fwd(x: Tensor, w1: Tensor, b1: Optional[Tensor], w2: Tensor, b2: Optional[Tensor], want_h: bool = False):
+    """y = GELU(x @ w1^T + b1) @ w2^T + b2 -> bf16 [..., C] in one kernel, equal to gemm(gemm(x, w1, b1, act=1), w2, b2).
+    C = x.shape[-1] in MLP_FUSED_C, w1 [4C, C], w2 [C, 4C].  want_h: return (y, h, gelu'(pre)) for the backward."""
+    x, w1, w2 = _chk(x, BF16, "x"), _chk(w1, BF16, "w1"), _chk(w2, BF16, "w2")
+    b1, b2 = _chk(b1, F32, "b1"), _chk(b2, F32, "b2")
+    C = x.shape[-1]
+    M = x.numel() // C
+    assert tuple(w1.shape) == (4 * C, C) and tuple(w2.shape) == (C, 4 * C), (x.shape, w1.shape, w2.shape)
+    y = torch.empty_like(x)
+    h = torch.empty(*x.shape[:-1], 4 * C, dtype=BF16, device=x.device) if want_h else None
+    pre = torch.empty_like(h) if want_h else None
+    _lib.call("esvit_mlp_fwd", _p(x), _p(w1), _p(b1), _p(w2), _p(b2), _p(y), _p(h), _p(pre), M, C, _stream())
+    return (y, h, pre) if want_h else y
+
+
 _wgrad_ws = {}
 
 

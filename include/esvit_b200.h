@@ -116,6 +116,12 @@ int esvit_gemm_mul_colsum2(const void* a, const void* b, const void* mult, void*
 int esvit_gemm_wgrad_ws_floats(int N, int K);
 int esvit_gemm_wgrad(const void* dy, const void* x, float* dw, float* ws, long long T, int N, int K, int accumulate,
                      int tile, void* stream);
+/* mlp_fwd: y[M,C] (bf16) = GELU(x[M,C] . w1[4C,C]^T + b1) . w2[C,4C]^T + b2 in one back-to-back wgmma kernel: the hidden
+ *   activation stays on chip.  h, gelu_grad [M,4C] bf16: both NULL (no-grad forward) or both set (they receive GELU(pre)
+ *   and gelu'(pre) for the backward).  Bit-identical to gemm_bf16 act 1 followed by gemm_bf16 act 0.  C in {96, 128, 192}
+ *   (other C: status 1001); biases fp32 or NULL; matrices 16-byte aligned. */
+int esvit_mlp_fwd(const void* x, const void* w1, const float* b1, const void* w2, const float* b2, void* y, void* h,
+                  void* gelu_grad, long long M, int C, void* stream);
 
 /* ---- GELU (exact erf), bf16 ------------------------------------------------ models/swin_transformer.py:21-37 */
 int esvit_gelu_fwd(const void* x, void* y, long long n, void* stream);
