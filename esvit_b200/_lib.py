@@ -61,6 +61,14 @@ SIGNATURES = {
     "esvit_region_match": [P, P, I, I, I, I, I, P, P, P],
     "esvit_mhsa_fwd": [P, P, P, I, I, I, I, F, P],
     "esvit_mhsa_bwd": [P, P, P, P, P, P, I, I, I, I, F, P],
+    "esvit_conv_im2col": [P, P, I, I, I, I, I, I, I, I, I, P],
+    "esvit_conv_col2im": [P, P, I, I, I, I, I, I, I, I, P],
+    "esvit_mhsa_win_fwd": [P, P, P, I, I, I, I, I, I, F, P],
+    "esvit_mhsa_win_bwd": [P, P, P, P, P, P, I, I, I, I, I, I, F, P],
+    "esvit_dwbn_fwd_stats": [P, P, P, P, P, I, I, I, I, I, I, P],
+    "esvit_dwbn_fwd_apply": [P, P, P, P, P, P, P, P, P, L, I, I, F, F, P],
+    "esvit_dwbn_bwd_stats": [P, P, P, P, P, P, P, L, I, P],
+    "esvit_dwbn_bwd_apply": [P, P, P, P, P, P, P, P, P, P, I, I, I, I, I, I, I, P],
     "esvit_vit_patches": [P, P, I, I, I, P],
     "esvit_vit_tokens_fwd": [P, P, P, P, I, I, I, P],
     "esvit_vit_tokens_bwd": [P, P, P, P, P, I, I, I, I, P],
@@ -147,6 +155,20 @@ _META = {
     "esvit_dino_ce_q_fwd": lambda a: {"rows": int(a[-3]), "K": int(a[-2])},
     "esvit_dino_ce_q_bwd": lambda a: {"rows": int(a[-3]), "K": int(a[-2])},
     "esvit_row_softmax_q": lambda a: {"rows": int(a[-3]), "K": int(a[-2])},
+    "esvit_conv_im2col": lambda a: {"B": int(a[3]), "C": int(a[4]), "H": int(a[5]), "W": int(a[6]), "k": int(a[7]),
+                                    "s": int(a[8]), "p": int(a[9]), "Kp": int(a[10])},
+    "esvit_conv_col2im": lambda a: {"B": int(a[2]), "C": int(a[3]), "H": int(a[4]), "W": int(a[5]), "k": int(a[6]),
+                                    "s": int(a[7]), "p": int(a[8]), "Kp": int(a[9])},
+    "esvit_dwbn_fwd_stats": lambda a: {"B": int(a[5]), "H": int(a[6]), "W": int(a[7]), "Hp": int(a[8]), "Wp": int(a[9]),
+                                       "C": int(a[10])},
+    "esvit_dwbn_fwd_apply": lambda a: {"N": int(a[9]), "C": int(a[10])},
+    "esvit_dwbn_bwd_stats": lambda a: {"N": int(a[7]), "C": int(a[8])},
+    "esvit_dwbn_bwd_apply": lambda a: {"B": int(a[10]), "H": int(a[11]), "W": int(a[12]), "Hp": int(a[13]),
+                                       "Wp": int(a[14]), "C": int(a[15])},
+    "esvit_mhsa_win_fwd": lambda a: {"B": int(a[3]), "H": int(a[4]), "W": int(a[5]), "w": int(a[6]), "C": int(a[7]),
+                                     "nH": int(a[8])},
+    "esvit_mhsa_win_bwd": lambda a: {"B": int(a[6]), "H": int(a[7]), "W": int(a[8]), "w": int(a[9]), "C": int(a[10]),
+                                     "nH": int(a[11])},
     "esvit_mhsa_fwd": lambda a: {"B": int(a[3]), "L": int(a[4]), "C": int(a[5]), "nH": int(a[6])},
     "esvit_mhsa_bwd": lambda a: {"B": int(a[6]), "L": int(a[7]), "C": int(a[8]), "nH": int(a[9])},
     "esvit_vit_tokens_bwd": lambda a: {"B": int(a[-5]), "N": int(a[-4]), "D": int(a[-3])},

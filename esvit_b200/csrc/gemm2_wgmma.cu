@@ -220,6 +220,15 @@ __device__ __forceinline__ float gelu_fwd_grad(float x, float& dy) {
   dy = fmaf(hx * m, nc, fmaf(0.5f, th, 0.5f));
   return fmaf(hx, th, hx);
 }
+// QuickGELU x sigmoid(1.702 x) (CvT's act_layer, models/cvt_v4_transformer.py:44-46) and its derivative
+// s (1 + 1.702 x (1 - s)), s = sigmoid(1.702 x)
+constexpr float QGELU_A = 1.702f;
+__device__ __forceinline__ float qgelu_fwd(float x) { return x * __frcp_rn(1.f + __expf(-QGELU_A * x)); }
+__device__ __forceinline__ float qgelu_fwd_grad(float x, float& dy) {
+  const float s = __frcp_rn(1.f + __expf(-QGELU_A * x));
+  dy = s * fmaf(QGELU_A * x, 1.f - s, 1.f);
+  return x * s;
+}
 
 struct Params {
   const float* bias;  // [N] or nullptr (EPI_BIAS / EPI_GELU)
@@ -258,8 +267,9 @@ struct Cfg {
   static_assert((2 * STAGES + 2 + 2 * NCHUNK) * 8 <= BAR_BYTES, "mbarrier area");
 };
 
-// map_o: out, map_x: gelu' out (EPI_GELU) or the multiplier in (EPI_MUL); both [64 columns x 64 rows] boxes, 128B swizzle
-template <int WG, int BN, int EPI, int AMN, int BMN>
+// map_o: out, map_x: gelu' out (EPI_GELU) or the multiplier in (EPI_MUL); both [64 columns x 64 rows] boxes, 128B swizzle.
+// QUICK (EPI_GELU only): QuickGELU instead of the tanh GELU
+template <int WG, int BN, int EPI, int AMN, int BMN, bool QUICK = false>
 __global__ void __launch_bounds__(128 * (WG + 1), 1) gemm_kernel(const __grid_constant__ CUtensorMap map_a,
                                                                  const __grid_constant__ CUtensorMap map_b,
                                                                  const __grid_constant__ CUtensorMap map_o,
@@ -483,9 +493,16 @@ __global__ void __launch_bounds__(128 * (WG + 1), 1) gemm_kernel(const __grid_co
               if constexpr (EPI == EPI_GELU) {
                 if (p.aux) {
                   float d0, d1;
-                  const float y0 = gelu_fwd_grad(v0, d0), y1 = gelu_fwd_grad(v1, d1);
+                  float y0, y1;
+                  if constexpr (QUICK) {
+                    y0 = qgelu_fwd_grad(v0, d0); y1 = qgelu_fwd_grad(v1, d1);
+                  } else {
+                    y0 = gelu_fwd_grad(v0, d0); y1 = gelu_fwd_grad(v1, d1);
+                  }
                   o[q] = pack_bf162(y0, y1);
                   d[q] = pack_bf162(d0, d1);
+                } else if constexpr (QUICK) {
+                  o[q] = pack_bf162(qgelu_fwd(v0), qgelu_fwd(v1));
                 } else {
                   o[q] = pack_bf162(gelu_fwd(v0), gelu_fwd(v1));
                 }
@@ -779,9 +796,19 @@ static bool make_map(CUtensorMap* map, const void* ptr, long long rows, long lon
   cuuint64_t strides[1] = {(cuuint64_t)cols * 2};
   cuuint32_t box[2] = {64u, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  return enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+  auto encode = [&]() {
+    return enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  };
+  CUresult r = encode();
+  if (r == CUDA_ERROR_INVALID_CONTEXT) {
+    // a driver-API call in a thread that has made no runtime call yet (e.g. the first GEMM of autograd's backward
+    // thread): the runtime binds its context to a thread lazily, so bind the current device's primary context and retry
+    int dev = 0;
+    if (cudaGetDevice(&dev) == cudaSuccess && cudaSetDevice(dev) == cudaSuccess) r = encode();
+  }
+  return r == CUDA_SUCCESS;
 }
 
 template <int C, bool STORE>
@@ -846,7 +873,7 @@ struct Call {
   Params p;
 };
 
-template <int WG, int BN, int EPI, int AMN, int BMN>
+template <int WG, int BN, int EPI, int AMN, int BMN, bool QUICK = false>
 static int launch_cfg(const Call& c, void* stream, int* rows_out) {
   using C = Cfg<WG, BN, EPI>;
   Params p = c.p;
@@ -864,7 +891,7 @@ static int launch_cfg(const Call& c, void* stream, int* rows_out) {
     if (!make_map(&mo, p.out, p.M, p.N, 64)) return ESVIT_ERR_BAD_ARG;
     if (p.aux && !make_map(&mx, p.aux, p.M, p.N, 64)) return ESVIT_ERR_BAD_ARG;
   }
-  auto kernel = gemm_kernel<WG, BN, EPI, AMN, BMN>;
+  auto kernel = gemm_kernel<WG, BN, EPI, AMN, BMN, QUICK>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM);
@@ -907,6 +934,16 @@ static int launch_epi(const Call& c, int wg, int bn, void* stream, int* rows_out
   return ESVIT_ERR_BAD_ARG;
 }
 
+// QuickGELU forward GEMM (K-major operands only: the CvT fc1)
+static int launch_quick(const Call& c, int wg, int bn, void* stream) {
+  if (c.a_mn || c.b_mn) return ESVIT_ERR_BAD_ARG;
+  if (wg == 2 && bn == 256) return launch_cfg<2, 256, EPI_GELU, 0, 0, true>(c, stream, nullptr);
+  if (wg == 2 && bn == 128) return launch_cfg<2, 128, EPI_GELU, 0, 0, true>(c, stream, nullptr);
+  if (wg == 1 && bn == 256) return launch_cfg<1, 256, EPI_GELU, 0, 0, true>(c, stream, nullptr);
+  if (wg == 1 && bn == 128) return launch_cfg<1, 128, EPI_GELU, 0, 0, true>(c, stream, nullptr);
+  return ESVIT_ERR_BAD_ARG;
+}
+
 static int launch(const Call& c, int epi, int wg, int bn, void* stream, int* rows_out = nullptr) {
   switch (epi) {
     case EPI_BIAS: return launch_epi<EPI_BIAS>(c, wg, bn, stream, rows_out);
@@ -946,18 +983,20 @@ static void pick_tile_wgrad(int Nout, int Kin, int tile, int* wg, int* bn) {
 // out[M,N] (bf16) = act( opA(a) . opB(b) + bias[N] )
 //   a: a_mn = 0: [M,K] row-major (K contiguous) | a_mn = 1: [K,M] row-major (M contiguous)
 //   b: b_mn = 0: [N,K] row-major (nn.Linear weight layout) | b_mn = 1: [K,N] row-major (N contiguous)
-//   act 0: identity; act 1: GELU (pre != NULL also receives gelu'(pre-activation) for the backward)
+//   act 0: identity; act 1: GELU (pre != NULL also receives gelu'(pre-activation) for the backward); act 2: QuickGELU
+//   x sigmoid(1.702 x) (pre likewise receives its derivative; a_mn = b_mn = 0 only)
 //   M, N, K multiples of 8; bias fp32 or NULL.  tile = 0 (automatic) or warpgroups * 1000 + BN (1128, 1256, 2128, 2256).
 ESVIT_API int esvit_gemm_bf16(const void* a, const void* b, const float* bias, void* out, void* pre, long long M, int N,
                               int K, int a_mn, int b_mn, int act, int tile, void* stream) {
-  if (M <= 0 || N <= 0 || K <= 0 || (N % 8) || (K % 8) || M > 0x7fffffffLL || (a_mn && (M % 8)) || act < 0 || act > 1)
+  if (M <= 0 || N <= 0 || K <= 0 || (N % 8) || (K % 8) || M > 0x7fffffffLL || (a_mn && (M % 8)) || act < 0 || act > 2)
     return ESVIT_ERR_BAD_ARG;
   hg::Call c;
   c.a = a; c.b = b; c.a_mn = a_mn ? 1 : 0; c.b_mn = b_mn ? 1 : 0;
-  c.p.bias = bias; c.p.out = (bf16*)out; c.p.aux = (act == 1) ? (bf16*)pre : nullptr; c.p.colsum = nullptr; c.p.part = nullptr;
+  c.p.bias = bias; c.p.out = (bf16*)out; c.p.aux = act ? (bf16*)pre : nullptr; c.p.colsum = nullptr; c.p.part = nullptr;
   c.p.M = (int)M; c.p.N = N; c.p.K = K; c.p.splits = 1; c.p.kb_per_split = (K + hg::BK - 1) / hg::BK;
   int wg, bn;
   hg::pick_tile(M, N, tile, &wg, &bn);
+  if (act == 2) return hg::launch_quick(c, wg, bn, stream);
   return hg::launch(c, act ? hg::EPI_GELU : hg::EPI_BIAS, wg, bn, stream);
 }
 

@@ -16,6 +16,12 @@
 //   dq     CTA = 64 queries: P = ex2(s' - lse'), dP = dO V^T, dS = P (dP - D), dQ = scale * dS K   (loop over key tiles)
 //   dkdv   CTA = 64 keys:    P^T, dV = P^T dO, dP^T = V dO^T, dS^T = P^T (dP^T - D), dK = scale * dS^T Q  (loop over queries)
 // Each output row is owned by exactly one warp.
+//
+// Window mode (WIN = true; CvT, models/cvt_v4_transformer.py Attention.forward :165-220): "sequence" s is window s of
+// the zero-padded Hp x Wp token map (images, then windows row-major, then tokens row-major), L = w*w <= 64 tokens.  q / k
+// / v rows are gathered from the token-major qkv [B*Hp*Wp, 3C] of the padded map; out / dout are the CROPPED map
+// [B*H*W, C]: padded query rows are not stored (their dO reads as 0, so their dq is 0), padded keys take part as in the
+// reference.  lse / dvec are [windows, nH, L] as in the dense mode.
 #include "wa_common.cuh"
 
 namespace mh {
@@ -101,6 +107,55 @@ __device__ __forceinline__ void store_rows(bf16* __restrict__ dst, long long ld,
   }
 }
 
+// window geometry of the WIN kernels (unused by the dense ones)
+struct Win {
+  int H, W, Hp, Wp, w, nwx, nwin;  // nwx windows per row, nwin per image
+};
+
+// padded-map row of token l of window s
+__device__ __forceinline__ long long win_row(const Win& g, int s, int l) {
+  const int img = s / g.nwin, wi = s - img * g.nwin, wy = wi / g.nwx, wx = wi - wy * g.nwx;
+  const int ty = l / g.w, tx = l - ty * g.w;
+  return ((long long)img * g.Hp + wy * g.w + ty) * g.Wp + wx * g.w + tx;
+}
+// cropped-map row of token l of window s, -1 for a padded position
+__device__ __forceinline__ long long win_out_row(const Win& g, int s, int l) {
+  const int img = s / g.nwin, wi = s - img * g.nwin, wy = wi / g.nwx, wx = wi - wy * g.nwx;
+  const int ty = l / g.w, tx = l - ty * g.w, y = wy * g.w + ty, x = wx * g.w + tx;
+  return (y < g.H && x < g.W) ? ((long long)img * g.H + y) * g.W + x : -1;
+}
+
+// load_tile for the rows of window s: src = row 0's column base, row r at (out ? cropped : padded) row of token r;
+// rows >= L and padded rows of the cropped map are zero
+template <bool OUT>
+__device__ __forceinline__ void load_tile_win(bf16* dst, const bf16* __restrict__ src, long long ld, const Win& g, int s,
+                                              int L) {
+#pragma unroll
+  for (int k = 0; k < 4; k++) {
+    const int e = threadIdx.x + k * NTHR;
+    const int r = e >> 3, c = (e & 7) * 8;
+    long long row = -1;
+    if (r < L) row = OUT ? win_out_row(g, s, r) : win_row(g, s, r);
+    const bool ok = row >= 0;
+    cp_async16(dst + r * LDS + c, src + (ok ? row * ld : 0) + c, ok ? 16 : 0);
+  }
+}
+
+// store_rows for window s: rows rA / rB < L go to (out ? cropped : padded) rows; padded rows of the cropped map skipped
+template <bool OUT>
+__device__ __forceinline__ void store_rows_win(bf16* __restrict__ dst, long long ld, const float (&o)[8][4], float s0,
+                                               float s1, int rA, int rB, int L, const Win& g, int s, int lane) {
+  long long oA = -1, oB = -1;
+  if (rA < L) oA = OUT ? win_out_row(g, s, rA) : win_row(g, s, rA);
+  if (rB < L) oB = OUT ? win_out_row(g, s, rB) : win_row(g, s, rB);
+#pragma unroll
+  for (int dt = 0; dt < 8; dt++) {
+    const int d = dt * 8 + (lane & 3) * 2;
+    if (oA >= 0) *reinterpret_cast<uint32_t*>(dst + oA * ld + d) = pack_bf162(o[dt][0] * s0, o[dt][1] * s0);
+    if (oB >= 0) *reinterpret_cast<uint32_t*>(dst + oB * ld + d) = pack_bf162(o[dt][2] * s1, o[dt][3] * s1);
+  }
+}
+
 __device__ __forceinline__ float quad_max(float v) {
   v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
   return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
@@ -111,19 +166,27 @@ __device__ __forceinline__ float quad_sum(float v) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+template <bool WIN>
 __global__ void __launch_bounds__(NTHR) mhsa_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out,
-                                                        float* __restrict__ lse, int L, int C, int nH, float c2) {
+                                                        float* __restrict__ lse, int L, int C, int nH, float c2,
+                                                        const Win win) {
   extern __shared__ __align__(16) unsigned char smraw[];
   bf16* Qs = reinterpret_cast<bf16*>(smraw);  // [Q | K0 | V0 | K1 | V1]
   const int q0 = blockIdx.x * 64, h = blockIdx.y, b = blockIdx.z;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const long long C3 = 3LL * C;
   const bf16* base = qkv + (long long)b * L * C3 + h * HD;
-  load_tile(Qs, base + q0 * C3, C3, L - q0);
-  load_tile(Qs + TILE, base + C, C3, L);
-  load_tile(Qs + 2 * TILE, base + 2 * C, C3, L);
+  if constexpr (WIN) {
+    load_tile_win<false>(Qs, qkv + h * HD, C3, win, b, L);
+    load_tile_win<false>(Qs + TILE, qkv + h * HD + C, C3, win, b, L);
+    load_tile_win<false>(Qs + 2 * TILE, qkv + h * HD + 2 * C, C3, win, b, L);
+  } else {
+    load_tile(Qs, base + q0 * C3, C3, L - q0);
+    load_tile(Qs + TILE, base + C, C3, L);
+    load_tile(Qs + 2 * TILE, base + 2 * C, C3, L);
+  }
   cp_async_commit();
-  const int nkt = (L + 63) / 64;
+  const int nkt = WIN ? 1 : (L + 63) / 64;
   float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
   float o[8][4];
 #pragma unroll
@@ -189,7 +252,10 @@ __global__ void __launch_bounds__(NTHR) mhsa_fwd_kernel(const bf16* __restrict__
   l0 = quad_sum(l0);
   l1 = quad_sum(l1);
   const int rA = q0 + warp * 16 + (lane >> 2), rB = rA + 8;
-  store_rows(out + (long long)b * L * C + h * HD, C, o, __fdividef(1.f, l0), __fdividef(1.f, l1), rA, rB, L, lane);
+  if constexpr (WIN)
+    store_rows_win<true>(out + h * HD, C, o, __fdividef(1.f, l0), __fdividef(1.f, l1), rA, rB, L, win, b, lane);
+  else
+    store_rows(out + (long long)b * L * C + h * HD, C, o, __fdividef(1.f, l0), __fdividef(1.f, l1), rA, rB, L, lane);
   if ((lane & 3) == 0) {
     float* lp = lse + ((long long)b * nH + h) * L;
     if (rA < L) lp[rA] = (m0 + lg2(l0)) * LN2;
@@ -198,14 +264,24 @@ __global__ void __launch_bounds__(NTHR) mhsa_fwd_kernel(const bf16* __restrict__
 }
 
 // D[b, h, i] = sum_d dO[b, i, h, d] * O[b, i, h, d]; one warp per token row, lanes over (head, dim pair)
+// (WIN: B windows; a padded query row has D = 0)
+template <bool WIN>
 __global__ void __launch_bounds__(256) mhsa_bwd_prep_kernel(const bf16* __restrict__ out, const bf16* __restrict__ dout,
-                                                            float* __restrict__ dvec, int B, int L, int C, int nH) {
+                                                            float* __restrict__ dvec, int B, int L, int C, int nH,
+                                                            const Win win) {
   const int lane = threadIdx.x & 31;
   const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
   if (row >= (long long)B * L) return;
   const int b = (int)(row / L), i = (int)(row - (long long)b * L);
+  long long orow = row;
+  if constexpr (WIN) orow = win_out_row(win, b, i);
   for (int h = 0; h < nH; h++) {
-    const long long off = row * C + h * HD + lane * 2;
+    if constexpr (WIN)
+      if (orow < 0) {
+        if (lane == 0) dvec[((long long)b * nH + h) * L + i] = 0.f;
+        continue;
+      }
+    const long long off = orow * C + h * HD + lane * 2;
     const float2 o = __bfloat1622float2(*reinterpret_cast<const bf162*>(out + off));
     const float2 g = __bfloat1622float2(*reinterpret_cast<const bf162*>(dout + off));
     const float d = warp_sum(o.x * g.x + o.y * g.y);
@@ -214,27 +290,35 @@ __global__ void __launch_bounds__(256) mhsa_bwd_prep_kernel(const bf16* __restri
 }
 
 // dQ of 64 query rows; lse / dvec as the forward / prep kernels wrote them
+template <bool WIN>
 __global__ void __launch_bounds__(NTHR) mhsa_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
                                                            const float* __restrict__ lse, const float* __restrict__ dvec,
                                                            bf16* __restrict__ dqkv, int L, int C, int nH, float c2,
-                                                           float scale) {
+                                                           float scale, const Win win) {
   extern __shared__ __align__(16) unsigned char smraw[];
   bf16* Qs = reinterpret_cast<bf16*>(smraw);  // [Q | dO | K0 | V0 | K1 | V1]
   const int q0 = blockIdx.x * 64, h = blockIdx.y, b = blockIdx.z;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const long long C3 = 3LL * C;
   const bf16* base = qkv + (long long)b * L * C3 + h * HD;
-  load_tile(Qs, base + q0 * C3, C3, L - q0);
-  load_tile(Qs + TILE, dout + ((long long)b * L + q0) * C + h * HD, C, L - q0);
-  load_tile(Qs + 2 * TILE, base + C, C3, L);
-  load_tile(Qs + 3 * TILE, base + 2 * C, C3, L);
+  if constexpr (WIN) {
+    load_tile_win<false>(Qs, qkv + h * HD, C3, win, b, L);
+    load_tile_win<true>(Qs + TILE, dout + h * HD, C, win, b, L);
+    load_tile_win<false>(Qs + 2 * TILE, qkv + h * HD + C, C3, win, b, L);
+    load_tile_win<false>(Qs + 3 * TILE, qkv + h * HD + 2 * C, C3, win, b, L);
+  } else {
+    load_tile(Qs, base + q0 * C3, C3, L - q0);
+    load_tile(Qs + TILE, dout + ((long long)b * L + q0) * C + h * HD, C, L - q0);
+    load_tile(Qs + 2 * TILE, base + C, C3, L);
+    load_tile(Qs + 3 * TILE, base + 2 * C, C3, L);
+  }
   cp_async_commit();
   const int rA = q0 + warp * 16 + (lane >> 2), rB = rA + 8;
   const float* lp = lse + ((long long)b * nH + h) * L;
   const float* dp = dvec + ((long long)b * nH + h) * L;
   const float lA = rA < L ? lp[rA] * LOG2E : 0.f, lB = rB < L ? lp[rB] * LOG2E : 0.f;
   const float DA = rA < L ? dp[rA] : 0.f, DB = rB < L ? dp[rB] : 0.f;
-  const int nkt = (L + 63) / 64;
+  const int nkt = WIN ? 1 : (L + 63) / 64;
   float dq[8][4];
 #pragma unroll
   for (int dt = 0; dt < 8; dt++) dq[dt][0] = dq[dt][1] = dq[dt][2] = dq[dt][3] = 0.f;
@@ -278,14 +362,18 @@ __global__ void __launch_bounds__(NTHR) mhsa_bwd_dq_kernel(const bf16* __restric
     __syncthreads();
   }
   cp_async_wait<0>();
-  store_rows(dqkv + (long long)b * L * C3 + h * HD, C3, dq, scale, scale, rA, rB, L, lane);
+  if constexpr (WIN)
+    store_rows_win<false>(dqkv + h * HD, C3, dq, scale, scale, rA, rB, L, win, b, lane);
+  else
+    store_rows(dqkv + (long long)b * L * C3 + h * HD, C3, dq, scale, scale, rA, rB, L, lane);
 }
 
 // dK, dV of 64 key rows
+template <bool WIN>
 __global__ void __launch_bounds__(NTHR) mhsa_bwd_dkdv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
                                                              const float* __restrict__ lse, const float* __restrict__ dvec,
                                                              bf16* __restrict__ dqkv, int L, int C, int nH, float c2,
-                                                             float scale) {
+                                                             float scale, const Win win) {
   extern __shared__ __align__(16) unsigned char smraw[];
   bf16* Ks = reinterpret_cast<bf16*>(smraw);            // [K | V | Q0 | dO0 | Q1 | dO1]
   float* stat = reinterpret_cast<float*>(Ks + 6 * TILE);  // [2 stages][lse' 64 | D 64]
@@ -296,17 +384,24 @@ __global__ void __launch_bounds__(NTHR) mhsa_bwd_dkdv_kernel(const bf16* __restr
   const bf16* gbase = dout + (long long)b * L * C + h * HD;
   const float* lp = lse + ((long long)b * nH + h) * L;
   const float* dp = dvec + ((long long)b * nH + h) * L;
-  load_tile(Ks, base + C + k0 * C3, C3, L - k0);
-  load_tile(Ks + TILE, base + 2 * C + k0 * C3, C3, L - k0);
-  load_tile(Ks + 2 * TILE, base, C3, L);
-  load_tile(Ks + 3 * TILE, gbase, C, L);
+  if constexpr (WIN) {
+    load_tile_win<false>(Ks, qkv + h * HD + C, C3, win, b, L);
+    load_tile_win<false>(Ks + TILE, qkv + h * HD + 2 * C, C3, win, b, L);
+    load_tile_win<false>(Ks + 2 * TILE, qkv + h * HD, C3, win, b, L);
+    load_tile_win<true>(Ks + 3 * TILE, dout + h * HD, C, win, b, L);
+  } else {
+    load_tile(Ks, base + C + k0 * C3, C3, L - k0);
+    load_tile(Ks + TILE, base + 2 * C + k0 * C3, C3, L - k0);
+    load_tile(Ks + 2 * TILE, base, C3, L);
+    load_tile(Ks + 3 * TILE, gbase, C, L);
+  }
   cp_async_commit();
   if (threadIdx.x < 64) {  // queries past L: lse' = +inf -> P = 0
     const int q = threadIdx.x;
     stat[q] = q < L ? lp[q] * LOG2E : INFINITY;
     stat[64 + q] = q < L ? dp[q] : 0.f;
   }
-  const int nqt = (L + 63) / 64;
+  const int nqt = WIN ? 1 : (L + 63) / 64;
   float dk[8][4], dv[8][4];
 #pragma unroll
   for (int dt = 0; dt < 8; dt++)
@@ -363,9 +458,14 @@ __global__ void __launch_bounds__(NTHR) mhsa_bwd_dkdv_kernel(const bf16* __restr
   }
   cp_async_wait<0>();
   const int rA = k0 + warp * 16 + (lane >> 2), rB = rA + 8;
-  bf16* dst = dqkv + (long long)b * L * C3 + h * HD;
-  store_rows(dst + C, C3, dk, scale, scale, rA, rB, L, lane);
-  store_rows(dst + 2 * C, C3, dv, 1.f, 1.f, rA, rB, L, lane);
+  if constexpr (WIN) {
+    store_rows_win<false>(dqkv + h * HD + C, C3, dk, scale, scale, rA, rB, L, win, b, lane);
+    store_rows_win<false>(dqkv + h * HD + 2 * C, C3, dv, 1.f, 1.f, rA, rB, L, win, b, lane);
+  } else {
+    bf16* dst = dqkv + (long long)b * L * C3 + h * HD;
+    store_rows(dst + C, C3, dk, scale, scale, rA, rB, L, lane);
+    store_rows(dst + 2 * C, C3, dv, 1.f, 1.f, rA, rB, L, lane);
+  }
 }
 
 constexpr size_t FWD_SMEM = 5 * TILE * sizeof(bf16);
@@ -383,33 +483,75 @@ static cudaError_t opt_in(K kernel, size_t smem) {
                           : cudaSuccess;
 }
 
+// window geometry of a B x H x W map in windows of w x w (rejects what the WIN kernels cannot address)
+static bool win_geo(int B, int H, int W, int w, Win* g, int* nwin_total) {
+  if (B < 1 || H < 1 || W < 1 || w < 1 || w * w > 64 || w > H || w > W) return false;
+  g->H = H; g->W = W; g->w = w;
+  g->Hp = (H + w - 1) / w * w; g->Wp = (W + w - 1) / w * w;
+  g->nwx = g->Wp / w; g->nwin = (g->Hp / w) * g->nwx;
+  const long long n = (long long)B * g->nwin;
+  if (n > 65535) return false;
+  *nwin_total = (int)n;
+  return true;
+}
+
+template <bool WIN>
+static int fwd_launch(const void* qkv, void* out, float* lse, int B, int L, int C, int nH, float scale, const Win& win,
+                      void* stream) {
+  const dim3 grid((L + 63) / 64, nH, B);
+  mhsa_fwd_kernel<WIN><<<grid, NTHR, FWD_SMEM, (cudaStream_t)stream>>>((const bf16*)qkv, (bf16*)out, lse, L, C, nH,
+                                                                       scale * LOG2E, win);
+  ESVIT_LAUNCH_CHECK();
+}
+
+template <bool WIN>
+static int bwd_launch(const void* qkv, const void* out, const void* dout, const float* lse, float* dvec, void* dqkv, int B,
+                      int L, int C, int nH, float scale, const Win& win, void* stream) {
+  cudaError_t e = opt_in(mhsa_bwd_dq_kernel<WIN>, DQ_SMEM);
+  if (e == cudaSuccess) e = opt_in(mhsa_bwd_dkdv_kernel<WIN>, DKDV_SMEM);
+  if (e != cudaSuccess) return (int)e;
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long rows = (long long)B * L;
+  mhsa_bwd_prep_kernel<WIN><<<(unsigned)((rows + 7) / 8), 256, 0, st>>>((const bf16*)out, (const bf16*)dout, dvec, B, L,
+                                                                        C, nH, win);
+  const dim3 grid((L + 63) / 64, nH, B);
+  const float c2 = scale * LOG2E;
+  mhsa_bwd_dq_kernel<WIN><<<grid, NTHR, DQ_SMEM, st>>>((const bf16*)qkv, (const bf16*)dout, lse, dvec, (bf16*)dqkv, L, C,
+                                                       nH, c2, scale, win);
+  mhsa_bwd_dkdv_kernel<WIN><<<grid, NTHR, DKDV_SMEM, st>>>((const bf16*)qkv, (const bf16*)dout, lse, dvec, (bf16*)dqkv, L,
+                                                           C, nH, c2, scale, win);
+  ESVIT_LAUNCH_CHECK();
+}
+
 }  // namespace mh
 
 ESVIT_API int esvit_mhsa_fwd(const void* qkv, void* out, float* lse, int B, int L, int C, int nH, float scale,
                              void* stream) {
   if (!mh::ok_args(qkv, out, B, L, C, nH) || !lse) return ESVIT_ERR_BAD_ARG;
-  const dim3 grid((L + 63) / 64, nH, B);
-  mh::mhsa_fwd_kernel<<<grid, mh::NTHR, mh::FWD_SMEM, (cudaStream_t)stream>>>(
-      (const bf16*)qkv, (bf16*)out, lse, L, C, nH, scale * mh::LOG2E);
-  ESVIT_LAUNCH_CHECK();
+  return mh::fwd_launch<false>(qkv, out, lse, B, L, C, nH, scale, mh::Win{}, stream);
 }
 
 ESVIT_API int esvit_mhsa_bwd(const void* qkv, const void* out, const void* dout, const float* lse, float* dvec,
                              void* dqkv, int B, int L, int C, int nH, float scale, void* stream) {
   if (!mh::ok_args(qkv, dqkv, B, L, C, nH) || !mh::ok_args(out, dout, B, L, C, nH) || !lse || !dvec)
     return ESVIT_ERR_BAD_ARG;
-  cudaError_t e = mh::opt_in(mh::mhsa_bwd_dq_kernel, mh::DQ_SMEM);
-  if (e == cudaSuccess) e = mh::opt_in(mh::mhsa_bwd_dkdv_kernel, mh::DKDV_SMEM);
-  if (e != cudaSuccess) return (int)e;
-  cudaStream_t st = (cudaStream_t)stream;
-  const long long rows = (long long)B * L;
-  mh::mhsa_bwd_prep_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>((const bf16*)out, (const bf16*)dout, dvec, B, L, C,
-                                                                      nH);
-  const dim3 grid((L + 63) / 64, nH, B);
-  const float c2 = scale * mh::LOG2E;
-  mh::mhsa_bwd_dq_kernel<<<grid, mh::NTHR, mh::DQ_SMEM, st>>>((const bf16*)qkv, (const bf16*)dout, lse, dvec,
-                                                              (bf16*)dqkv, L, C, nH, c2, scale);
-  mh::mhsa_bwd_dkdv_kernel<<<grid, mh::NTHR, mh::DKDV_SMEM, st>>>((const bf16*)qkv, (const bf16*)dout, lse, dvec,
-                                                                  (bf16*)dqkv, L, C, nH, c2, scale);
-  ESVIT_LAUNCH_CHECK();
+  return mh::bwd_launch<false>(qkv, out, dout, lse, dvec, dqkv, B, L, C, nH, scale, mh::Win{}, stream);
+}
+
+ESVIT_API int esvit_mhsa_win_fwd(const void* qkv, void* out, float* lse, int B, int H, int W, int w, int C, int nH,
+                                 float scale, void* stream) {
+  mh::Win g;
+  int nw;
+  if (!mh::win_geo(B, H, W, w, &g, &nw) || !mh::ok_args(qkv, out, nw, w * w, C, nH) || !lse) return ESVIT_ERR_BAD_ARG;
+  return mh::fwd_launch<true>(qkv, out, lse, nw, w * w, C, nH, scale, g, stream);
+}
+
+ESVIT_API int esvit_mhsa_win_bwd(const void* qkv, const void* out, const void* dout, const float* lse, float* dvec,
+                                 void* dqkv, int B, int H, int W, int w, int C, int nH, float scale, void* stream) {
+  mh::Win g;
+  int nw;
+  if (!mh::win_geo(B, H, W, w, &g, &nw) || !mh::ok_args(qkv, dqkv, nw, w * w, C, nH) ||
+      !mh::ok_args(out, dout, nw, w * w, C, nH) || !lse || !dvec)
+    return ESVIT_ERR_BAD_ARG;
+  return mh::bwd_launch<true>(qkv, out, dout, lse, dvec, dqkv, nw, w * w, C, nH, scale, g, stream);
 }

@@ -20,6 +20,7 @@ import torch.distributed as dist
 from . import ops, utils
 from .losses import DDINOLoss, DINOLoss
 from .optim import FusedAdamWEMA
+from . import cvt_v4_transformer as cvts
 from . import vision_transformer as vits
 from .swin_transformer import SwinTransformer
 from .vision_transformer import DINOHead
@@ -39,16 +40,25 @@ VIT_SPECS = {
     "vit_base_p16": dict(vit_arch="vit_base", patch_size=16, drop_path_rate=0.1),
 }
 
+# CvT (main_esvit.py:280-301 with experiments/imagenet/cvt_v4/s1.yaml): `cvt_spec` is the MODEL.SPEC
+CVT_SPECS = {
+    "cvt_13": dict(cvt_spec=cvts.S1_SPEC, drop_path_rate=0.1),
+}
+
 
 def build_network(spec: dict, out_dim: int, use_dense_prediction: bool, is_teacher: bool = False,
                   norm_last_layer: bool = True, img_size: int = 224, head_kwargs: Optional[dict] = None) -> nn.Module:
-    """What main_esvit.py:235-254 (Swin) / :304-327 (ViT, a spec with `vit_arch`) builds: the backbone (teacher:
+    """What main_esvit.py:235-254 (Swin) / :304-327 (ViT, a spec with `vit_arch`) / :280-301 (CvT, a spec with
+    `cvt_spec`) builds: the backbone (teacher:
     drop_path 0) + DINOHead(s) assigned to ``.head`` / ``.head_dense``."""
     spec = dict(spec)
     if is_teacher:
         spec["drop_path_rate"] = 0.0
     vit_arch = spec.pop("vit_arch", None)
-    if vit_arch is not None:
+    cvt_spec = spec.pop("cvt_spec", None)
+    if cvt_spec is not None:
+        net = cvts.cvt(cvt_spec, 0, use_dense_prediction, drop_path_rate=spec["drop_path_rate"])
+    elif vit_arch is not None:
         net = vits.__dict__[vit_arch](img_size=[img_size], use_dense_prediction=use_dense_prediction, **spec)
     else:
         net = SwinTransformer(img_size=img_size, in_chans=3, num_classes=0, patch_size=4, mlp_ratio=4., qkv_bias=True,
@@ -242,7 +252,9 @@ def make_step(arch: str = "swin_tiny_w7", out_dim: int = 65536, ncrops: int = 10
               teacher_temp: float = 0.04, seed: int = 0, optimizer: str = "fused", cuda_graph: bool = False):
     """Build student/teacher/loss/optimizer the way train_esvit does (main_esvit.py:235-435) and return
     (step, student, teacher, loss)."""
-    spec = dict(spec if spec is not None else (VIT_SPECS[arch] if arch in VIT_SPECS else SWIN_SPECS[arch]))
+    if spec is None:
+        spec = VIT_SPECS.get(arch) or CVT_SPECS.get(arch) or SWIN_SPECS[arch]
+    spec = dict(spec)
     if drop_path is not None:
         spec["drop_path_rate"] = drop_path
     torch.manual_seed(seed)

@@ -69,14 +69,15 @@ class LinearFn(Function):
 class MlpFn(Function):
     """fc2(gelu(fc1(x))) (models/swin_transformer.py:31-35).  forward at C in ops.MLP_FUSED_C (Swin stages 0-1): ONE
     back-to-back kernel (esvit_mlp_fwd) writes y and, when a gradient is needed, h and gelu'; at other C: h, gelu' from ONE
-    GEMM (bias + exact GELU epilogue), y = h . W2^T + b2.  backward: d(pre) = (dy . W2) * gelu' with the fc1 bias gradient
+    GEMM (bias + exact GELU epilogue), y = h . W2^T + b2.  act 2 (CvT's QuickGELU FeedForward) always takes the two-GEMM
+    path with the QuickGELU epilogue; its derivative is the stored multiplier, so the backward is the same.  backward: d(pre) = (dy . W2) * gelu' with the fc1 bias gradient
     as column sums, all in one GEMM epilogue; dx = d(pre) . W1; dW1, dW2 in fp32.  b2's gradient is produced by the consumer (residual add + LN backward)."""
 
     @staticmethod
-    def forward(ctx, x, w1p, w1, b1, w2p, w2, b2):
+    def forward(ctx, x, w1p, w1, b1, w2p, w2, b2, act: int = 1):
         need = any(ctx.needs_input_grad)  # (grad mode is always off inside Function.forward: needs_input_grad is the signal)
         C = x.shape[-1]
-        if C in ops.MLP_FUSED_C and w1.shape[0] == 4 * C:
+        if act == 1 and C in ops.MLP_FUSED_C and w1.shape[0] == 4 * C:
             # one back-to-back kernel: h goes to HBM only when the backward needs it, and is never read back here
             if need:
                 y, h, pre = ops.mlp_fwd(x, w1, b1, w2, b2, want_h=True)
@@ -84,9 +85,9 @@ class MlpFn(Function):
                 y, h, pre = ops.mlp_fwd(x, w1, b1, w2, b2), None, None
         else:
             if need:
-                h, pre = ops.gemm(x, w1, b1, act=1, want_pre=True)
+                h, pre = ops.gemm(x, w1, b1, act=act, want_pre=True)
             else:
-                h, pre = ops.gemm(x, w1, b1, act=1), None
+                h, pre = ops.gemm(x, w1, b1, act=act), None
             y = ops.gemm(h, w2, b2)
         ctx.save_for_backward(x, w1, w2, pre, h)
         ctx.keys = (("w", w1p.data_ptr()), tuple(w1p.shape), ("w", w2p.data_ptr()), tuple(w2p.shape))
@@ -106,7 +107,7 @@ class MlpFn(Function):
         dpre = ops.gemm_mul_colsum(g2, w2, pre.reshape(-1, Nh), db1, b_mn=True)      # W2 [C, 4C] read as it lies
         dx = ops.gemm(dpre, w1, None, b_mn=True).view(x.shape) if ctx.needs_input_grad[0] else None
         dw1 = _wgrad(k1, dpre, x.reshape(-1, x.shape[-1]), s1) if ctx.needs_input_grad[1] else None
-        return dx, dw1, None, (db1 if first else None), dw2, None, None
+        return dx, dw1, None, (db1 if first else None), dw2, None, None, None
 
 
 class HeadMlpFn(Function):

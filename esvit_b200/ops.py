@@ -1164,6 +1164,180 @@ def region_match(s_fea: Tensor, t_fea: Tensor, B: int, ncrops: int, Tg: int, Tl:
 
 
 # ------------------------------------------------------------------------------------------------------------
+# CvT (models/cvt_v4_transformer.py): conv token embedding, depthwise conv + BatchNorm, window attention at head dim 64.
+# A window group g = (B, H, W, w, row0, prow0): B maps of H x W tokens at rows [row0, row0 + B*H*W) of the token-major
+# stream, their zero-padded Hp x Wp maps (multiples of the window w) at rows [prow0, prow0 + B*Hp*Wp) of the padded
+# buffers (the depthwise + BN output and the qkv GEMM output).
+
+
+def win_padded(H: int, W: int, w: int) -> Tuple[int, int]:
+    return -(-H // w) * w, -(-W // w) * w
+
+
+def conv_out_size(S: int, k: int, stride: int, pad: int) -> int:
+    return (S + 2 * pad - k) // stride + 1
+
+
+class ConvEmbedFn(Function):
+    """Conv2d(Cin, Cout, k, stride, pad) of ConvEmbed (:349-382) over every resolution group as ONE GEMM: the patch rows
+    bf16 [sum B*Ho*Wo, Kp] (esvit_conv_im2col) . w16^T + bias -> bf16 [sum B*Ho*Wo, Cout], groups back to back.
+    Source: `imgs` (fp32 NCHW crops, one tensor per group; no input gradient) or x fp32 token-major [T, Cin] with
+    groups ((B, H, W, row0), ...).  w16 bf16 [Cout, Kp]: the weight flattened in (c, ky, kx) order, K padded to a multiple
+    of 8 with zero columns.  bias (fp32 [Cout]) gets its gradient from the consumer (the fused add + LN).  backward: the
+    fp32 weight gradient (padding columns dropped) and, for x, the col2im gather of the rows' gradient."""
+
+    @staticmethod
+    def forward(ctx, x, weight, w16, bias, imgs, groups, k: int, stride: int, pad: int):
+        w16 = _chk(w16, BF16, "w16")
+        Cout, Kp = w16.shape
+        Cin = weight.shape[1]
+        if imgs is not None:
+            src = [(_chk(im, F32, "img"), 1, im.shape[0], im.shape[2], im.shape[3]) for im in imgs]
+        else:
+            x = _chk(x, F32, "x")
+            src = [(x, 0, B, H, W, r0) for B, H, W, r0 in groups]
+        n = [s[2] * conv_out_size(s[3], k, stride, pad) * conv_out_size(s[4], k, stride, pad) for s in src]
+        rows = torch.empty(sum(n), Kp, dtype=BF16, device=w16.device)
+        r0 = 0
+        for s, ni in zip(src, n):
+            t, nchw, B, H, W = s[:5]
+            base = _p(t) if nchw else _po(t, s[5] * Cin)
+            _lib.call("esvit_conv_im2col", base, _po(rows, r0 * Kp), nchw, B, Cin, H, W, k, stride, pad, Kp, _stream())
+            r0 += ni
+        y = gemm(rows, w16, bias)
+        ctx.save_for_backward(rows, w16)
+        ctx.meta = (tuple(weight.shape), None if imgs is not None else (tuple(x.shape), tuple(groups)), k, stride, pad)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        rows, w16 = ctx.saved_tensors
+        wshape, xmeta, k, stride, pad = ctx.meta
+        g = _chk(g, BF16, "g")
+        Cout, Cin = wshape[0], wshape[1]
+        K = Cin * k * k
+        dw = None
+        if ctx.needs_input_grad[1]:
+            dw = gemm_wgrad(g, rows)
+            dw = (dw[:, :K].contiguous() if dw.shape[1] != K else dw).view(wshape)
+        dx = None
+        if xmeta is not None and ctx.needs_input_grad[0]:
+            xshape, groups = xmeta
+            drows = gemm(g, w16, None, b_mn=True)
+            Kp = drows.shape[1]
+            dx = torch.empty(xshape, dtype=F32, device=g.device)
+            o0 = 0
+            for B, H, W, r0 in groups:
+                _lib.call("esvit_conv_col2im", _po(drows, o0 * Kp), _po(dx, r0 * Cin), B, Cin, H, W, k, stride, pad, Kp,
+                          _stream())
+                o0 += B * conv_out_size(H, k, stride, pad) * conv_out_size(W, k, stride, pad)
+        return dx, dw, None, None, None, None, None, None, None
+
+
+def _bn_part(groups, C: int, device) -> Tensor:
+    n = max(-(-(B * Hp * Wp) // 256) for B, H, W, w, _, _ in groups for Hp, Wp in (win_padded(H, W, w),))
+    return torch.empty(n * 9 * C, dtype=F32, device=device)
+
+
+class DwBnFn(Function):
+    """DepthWiseConv2d.dw + .bn (:101-104) on the zero-padded maps (Attention.forward :170-180): y bf16 [T, C] (the
+    PreNorm output of every window group) -> bf16 [Tp, C] of the padded maps, ready for the pw GEMM.  `bn` is the
+    nn.BatchNorm2d holding gamma / beta and the running buffers; train: per-group batch statistics over the padded maps
+    (the running statistics are updated in place, group by group, as the reference's per-group forward does); else the
+    running statistics.  pg: the process group of a SyncBatchNorm (world size > 1) or None; the per-channel sums (and
+    the count) are then all-reduced in one call per BN call, forward and backward."""
+
+    @staticmethod
+    def forward(ctx, y, weight, gamma, beta, bn, groups, train: bool, pg):
+        y = _chk(y, BF16, "y")
+        w = _chk(weight, F32, "weight").view(-1, 9)
+        gamma, beta = _chk(gamma, F32, "gamma"), _chk(beta, F32, "beta")
+        C = y.shape[1]
+        Tp = sum(B * Hp * Wp for B, H, W, w_, _, _ in groups for Hp, Wp in (win_padded(H, W, w_),))
+        z = torch.empty(Tp, C, dtype=BF16, device=y.device)
+        out = torch.empty_like(z)
+        part = _bn_part(groups, C, y.device)
+        sums = torch.empty(len(groups), 2 * C + 1, dtype=torch.float64, device=y.device)
+        stat = torch.empty(len(groups), 4 * C, dtype=F32, device=y.device)
+        rm, rv, nbt = bn.running_mean, bn.running_var, bn.num_batches_tracked
+        for i, (B, H, W, w_, r0, p0) in enumerate(groups):
+            Hp, Wp = win_padded(H, W, w_)
+            _lib.call("esvit_dwbn_fwd_stats", _po(y, r0 * C), _p(w), _po(z, p0 * C), _p(part), _p(sums[i]), B, H, W,
+                      Hp, Wp, C, _stream())
+            if train and pg is not None:
+                torch.distributed.all_reduce(sums[i], group=pg)
+            _lib.call("esvit_dwbn_fwd_apply", _po(z, p0 * C), _p(gamma), _p(beta), _p(sums[i]) if train else None,
+                      _p(rm), _p(rv), _p(nbt) if (train and nbt is not None) else None, _p(stat[i]), _po(out, p0 * C),
+                      B * Hp * Wp, C, 1 if train else 0, float(bn.momentum), float(bn.eps), _stream())
+        ctx.save_for_backward(y, z, w, stat)
+        ctx.meta = (tuple(groups), train, pg, tuple(weight.shape), gamma.data_ptr(), weight.data_ptr())
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        y, z, w, stat = ctx.saved_tensors
+        groups, train, pg, wshape, gptr, wptr = ctx.meta
+        g = _chk(g, BF16, "g")
+        C = y.shape[1]
+        dy = torch.empty_like(y)
+        part = _bn_part(groups, C, y.device)
+        bsums = torch.empty(2 * C + 1, dtype=torch.float64, device=y.device)
+        coef = torch.empty(3 * C, dtype=F32, device=y.device)
+        dwt, first_w = _acc(("dw", wptr), wshape, y.device)
+        aff, first_a = _acc(("bn", gptr), (2, C), y.device)  # dgamma | dbeta
+        for i, (B, H, W, w_, r0, p0) in enumerate(groups):
+            Hp, Wp = win_padded(H, W, w_)
+            N = B * Hp * Wp
+            _lib.call("esvit_dwbn_bwd_stats", _po(g, p0 * C), _po(z, p0 * C), _p(stat[i]), _p(part), _p(bsums),
+                      _p(aff[0]), _p(aff[1]), N, C, _stream())
+            if train and pg is not None:
+                torch.distributed.all_reduce(bsums, group=pg)
+            _lib.call("esvit_dwbn_bwd_apply", _po(g, p0 * C), _po(z, p0 * C), _po(y, r0 * C), _p(w), _p(stat[i]),
+                      _p(bsums), _p(coef), _po(dy, r0 * C), _p(part), _p(dwt), B, H, W, Hp, Wp, C, 1 if train else 0,
+                      _stream())
+        return (dy, dwt if first_w else None, aff[0] if first_a else None, aff[1] if first_a else None,
+                None, None, None, None)
+
+
+class MhsaWinGroupsFn(Function):
+    """Window attention of CvT (Attention.forward :180-218; no mask, no bias) at head dim 64: qkv bf16 [Tp, 3C] of the
+    padded maps (pw GEMM output incl. bias) -> the cropped output bf16 [T, C]; groups as DwBnFn's.  One launch per group.
+    qkv_bias only receives its gradient: the fixed-order column sums of dqkv."""
+
+    @staticmethod
+    def forward(ctx, qkv, qkv_bias, groups, num_heads: int, scale: float):
+        qkv = _chk(qkv, BF16, "qkv")
+        Tp, C3 = qkv.shape
+        C = C3 // 3
+        T = sum(B * H * W for B, H, W, _, _, _ in groups)
+        out = torch.empty(T, C, dtype=BF16, device=qkv.device)
+        lse = torch.empty(Tp * num_heads, dtype=F32, device=qkv.device)  # per group [windows, nH, w*w] at prow0 * nH
+        for B, H, W, w, r0, p0 in groups:
+            _lib.call("esvit_mhsa_win_fwd", _po(qkv, p0 * C3), _po(out, r0 * C), _po(lse, p0 * num_heads), B, H, W, w, C,
+                      num_heads, scale, _stream())
+        ctx.save_for_backward(qkv, out, lse)
+        ctx.meta = (tuple(groups), num_heads, scale, qkv_bias is not None)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        qkv, out, lse = ctx.saved_tensors
+        groups, nH, scale, has_bias = ctx.meta
+        g = _chk(g, BF16, "g")
+        C3 = qkv.shape[1]
+        C = C3 // 3
+        dqkv = torch.empty_like(qkv)
+        dvec = torch.empty_like(lse)
+        for B, H, W, w, r0, p0 in groups:
+            _lib.call("esvit_mhsa_win_bwd", _po(qkv, p0 * C3), _po(out, r0 * C), _po(g, r0 * C), _po(lse, p0 * nH),
+                      _po(dvec, p0 * nH), _po(dqkv, p0 * C3), B, H, W, w, C, nH, scale, _stream())
+        return dqkv, (colsum(dqkv) if has_bias else None), None, None, None
+
+
+# ------------------------------------------------------------------------------------------------------------
 # optimiser-side multi-tensor ops
 
 

@@ -105,7 +105,8 @@ int esvit_gemm_mul_colsum(const void* a, const void* w, const void* mult, void* 
  * row-major matrices read "transposed" by TMA + wgmma's transpose bits: no transposed copies).
  * gemm_bf16: out[M,N] (bf16) = act(opA(a) . opB(b) + bias[N]).  a: a_mn = 0 [M,K] | a_mn = 1 [K,M];  b: b_mn = 0 [N,K]
  *   (Linear weight, forward) | b_mn = 1 [K,N] (Linear weight [out = K, in = N], input gradient).  act 0 identity, 1 exact
- *   GELU (pre != NULL also receives gelu'(pre-activation)).  tile: 0 = automatic, else warpgroups * 1000 + BN.
+ *   GELU (pre != NULL also receives gelu'(pre-activation)); act 2: QuickGELU x sigmoid(1.702 x) (pre likewise; a_mn =
+ *   b_mn = 0 only).  tile: 0 = automatic, else warpgroups * 1000 + BN.
  * gemm_mul_colsum2: out = (a . opB(b)) * mult, colsum ACCUMULATED (see esvit_gemm_mul_colsum); ws fp32 [160 * N].
  * gemm_wgrad: dw[N,K] (fp32) (+)= dy[T,N]^T . x[T,K], split over T, deterministic fold of fp32 partial tiles held in ws
  *   (esvit_gemm_wgrad_ws_floats(N, K) fp32 elements).  All of M / N / K / T multiples of 8. */
@@ -209,6 +210,39 @@ int esvit_vit_tokens_fwd(const void* pe, const float* cls, const float* pos, flo
 int esvit_vit_tokens_bwd(const float* g, void* dpe, float* dpos, float* dbias, float* dcls, int accumulate, int B, int N,
                          int D, void* stream);
 int esvit_vit_split(float* x, float* cls, float* region, int B, int N, int D, int dir, void* stream);
+
+/* ---- CvT (models/cvt_v4_transformer.py) ------------------------------------------------------------------------------
+ * conv_im2col: x fp32 NCHW [B, C, H, W] (nchw = 1) or token-major [B*H*W, C] (nchw = 0) -> rows bf16 [B*Ho*Wo, Kp] of a
+ *   k x k / stride / pad conv in the weight's (c, ky, kx) order, columns >= C*k*k zero; Kp % 8 == 0.
+ * conv_col2im: the transpose: drows bf16 [B*Ho*Wo, Kp] -> dx fp32 token-major [B*H*W, C] (written), fixed-order gather.
+ * mhsa_win_fwd / _bwd: esvit_mhsa_fwd / _bwd over the w x w windows of the zero-padded map (Hp, Wp = H, W rounded up to
+ *   multiples of w; w*w <= 64): qkv / dqkv bf16 [B*Hp*Wp, 3C], out / dout bf16 [B*H*W, C] (padded rows not stored / read
+ *   as zero), lse / dvec fp32 [B * windows, nH, w*w].
+ * dwbn_*: depthwise 3x3 conv (pad 1, no bias; w fp32 [C, 9]) of y bf16 [B*H*W, C] zero-padded to Hp x Wp, then
+ *   BatchNorm2d; C % 64 == 0.  fwd_stats: z bf16 [B*Hp*Wp, C] (conv output), sums fp64 [2C + 1] = (sum z, sum z^2, count).
+ *   fwd_apply: stat fp32 [4C] = (mean, rstd, gamma rstd, beta - mean gamma rstd) from sums (train: run_mean / run_var /
+ *   nbt updated in place when given) or from run_mean / run_var (train = 0); out bf16 [N, C] = z * stat[2] + stat[3].
+ *   bwd_stats: sums fp64 [2C + 1] = (sum dy, sum dy xhat, count); dbeta / dgamma fp32 [C] += the local sums.
+ *   bwd_apply: dx bf16 [B*H*W, C] (written), dw fp32 [C, 9] += filter gradient; coef fp32 [3C] scratch.
+ *   part: fp32 scratch of ceil(B*Hp*Wp / 256) * 9 * C floats.  No floating-point atomics. */
+int esvit_conv_im2col(const float* x, void* rows, int nchw, int B, int C, int H, int W, int k, int stride, int pad, int Kp,
+                      void* stream);
+int esvit_conv_col2im(const void* rows, float* dx, int B, int C, int H, int W, int k, int stride, int pad, int Kp,
+                      void* stream);
+int esvit_mhsa_win_fwd(const void* qkv, void* out, float* lse, int B, int H, int W, int w, int C, int nH, float scale,
+                       void* stream);
+int esvit_mhsa_win_bwd(const void* qkv, const void* out, const void* dout, const float* lse, float* dvec, void* dqkv,
+                       int B, int H, int W, int w, int C, int nH, float scale, void* stream);
+int esvit_dwbn_fwd_stats(const void* y, const float* w, void* z, float* part, double* sums, int B, int H, int W, int Hp,
+                         int Wp, int C, void* stream);
+int esvit_dwbn_fwd_apply(const void* z, const float* gamma, const float* beta, const double* sums, float* run_mean,
+                         float* run_var, long long* nbt, float* stat, void* out, long long N, int C, int train,
+                         float momentum, float eps, void* stream);
+int esvit_dwbn_bwd_stats(const void* dy, const void* z, const float* stat, float* part, double* sums, float* dgamma,
+                         float* dbeta, long long N, int C, void* stream);
+int esvit_dwbn_bwd_apply(const void* dy, const void* z, const void* y, const float* w, const float* stat,
+                         const double* sums, float* coef, void* dx, float* part, float* dw, int B, int H, int W, int Hp,
+                         int Wp, int C, int train, void* stream);
 
 /* ---- optimiser-side multi-tensor kernels (host arrays of device pointers) ----------------------------------
  * ema_multi: teacher = teacher*m + student*(1-m), bit-exact with main_esvit.py:587-590.
