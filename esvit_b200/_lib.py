@@ -69,6 +69,9 @@ SIGNATURES = {
     "esvit_dwbn_fwd_apply": [P, P, P, P, P, P, P, P, P, L, I, I, F, F, P],
     "esvit_dwbn_bwd_stats": [P, P, P, P, P, P, P, L, I, P],
     "esvit_dwbn_bwd_apply": [P, P, P, P, P, P, P, P, P, P, I, I, I, I, I, I, I, P],
+    "esvit_vil_sc_ws_floats": [I, I, I, I],
+    "esvit_vil_sc_fwd": [P, P, P, P, P, P, P, P, I, I, I, I, F, P],
+    "esvit_vil_sc_bwd": [P, P, P, P, P, P, P, P, P, P, P, P, P, P, P, I, I, I, I, F, P],
     "esvit_vit_patches": [P, P, I, I, I, P],
     "esvit_vit_tokens_fwd": [P, P, P, P, I, I, I, P],
     "esvit_vit_tokens_bwd": [P, P, P, P, P, I, I, I, I, P],
@@ -169,6 +172,8 @@ _META = {
                                      "nH": int(a[8])},
     "esvit_mhsa_win_bwd": lambda a: {"B": int(a[6]), "H": int(a[7]), "W": int(a[8]), "w": int(a[9]), "C": int(a[10]),
                                      "nH": int(a[11])},
+    "esvit_vil_sc_fwd": lambda a: {"B": int(a[8]), "nx": int(a[9]), "ny": int(a[10]), "nH": int(a[11])},
+    "esvit_vil_sc_bwd": lambda a: {"B": int(a[15]), "nx": int(a[16]), "ny": int(a[17]), "nH": int(a[18])},
     "esvit_mhsa_fwd": lambda a: {"B": int(a[3]), "L": int(a[4]), "C": int(a[5]), "nH": int(a[6])},
     "esvit_mhsa_bwd": lambda a: {"B": int(a[6]), "L": int(a[7]), "C": int(a[8]), "nH": int(a[9])},
     "esvit_vit_tokens_bwd": lambda a: {"B": int(a[-5]), "N": int(a[-4]), "D": int(a[-3])},

@@ -1337,6 +1337,65 @@ class MhsaWinGroupsFn(Function):
         return dqkv, (colsum(dqkv) if has_bias else None), None, None, None
 
 
+VIL_W = 7               # sliding-chunk size of the Vision Longformer
+VIL_NB = 1 + 9 * VIL_W * VIL_W  # local bias columns: the global key, then 9 neighbour chunks of 49 keys
+_vil_ws = {}  # scratch per geometry, never freed: a captured CUDA graph may still write into it
+
+
+class SlidingChunkAttnFn(Function):
+    """Vision Longformer attention with one global token (layers/longformer2d.py Long2DSCSelfAttention.forward
+    :139-330, exact = 0, rpe, shared global weights, head dim 32): q bf16 [B*N, C] (query GEMM output over all N = 1 +
+    nx*ny rows per image, unscaled), kv bf16 [B*N, 2C] -> the context bf16 [B*N, C] that feeds proj (global row 0
+    first, :330).  bias fp32 [nH, 49, 442] is the dense local bias (column 0: g2l[1]; 1 + j*49 + r: key r of neighbour
+    chunk j in slidingchunk_qk order), bias_g fp32 [nH, N] the global row's (g2g | g2l[0]).  mode is an int32 CUDA
+    tensor [1] holding 0 (all nine chunks), 1..8 (the own chunk plus mode_dict[mode]) or -1 (the own chunk only); the
+    kernels read it at run time (clamping it into -1..8), so a captured CUDA graph follows whatever was written into it
+    before the replay."""
+
+    @staticmethod
+    def forward(ctx, q, kv, bias, bias_g, mode, B: int, nx: int, ny: int, num_heads: int, scale: float):
+        q = _chk(q, BF16, "q")
+        kv = _chk(kv, BF16, "kv")
+        bias = _chk(bias, F32, "bias").contiguous()
+        bias_g = _chk(bias_g, F32, "bias_g").contiguous()
+        mode = _chk(mode, torch.int32, "mode")
+        N, C = 1 + nx * ny, 32 * num_heads
+        if q.shape != (B * N, C) or kv.shape != (B * N, 2 * C) or not q.is_contiguous() or not kv.is_contiguous():
+            raise ValueError(f"q [B*N, C] = [{B * N}, {C}] and kv [B*N, 2C] contiguous required, got "
+                             f"{tuple(q.shape)}, {tuple(kv.shape)}")
+        if bias.shape != (num_heads, VIL_W * VIL_W, VIL_NB) or bias_g.shape != (num_heads, N) or mode.numel() != 1:
+            raise ValueError("bias [nH, 49, 442], bias_g [nH, N] and a one-element mode required")
+        mx, my = -(-nx // VIL_W), -(-ny // VIL_W)
+        out = torch.empty(B * N, C, dtype=BF16, device=q.device)
+        lse = torch.empty(B * num_heads * mx * my * VIL_W * VIL_W, dtype=F32, device=q.device)
+        lse_g = torch.empty(B * num_heads, dtype=F32, device=q.device)
+        _lib.call("esvit_vil_sc_fwd", _p(q), _p(kv), _p(bias), _p(bias_g), _p(mode), _p(out), _p(lse), _p(lse_g), B, nx,
+                  ny, num_heads, scale, _stream())
+        ctx.save_for_backward(q, kv, bias, bias_g, mode, out, lse, lse_g)
+        ctx.meta = (B, nx, ny, num_heads, scale)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        q, kv, bias, bias_g, mode, out, lse, lse_g = ctx.saved_tensors
+        B, nx, ny, nH, scale = ctx.meta
+        g = _chk(g, BF16, "g").contiguous()
+        key = (q.device, B, nx, ny, nH)
+        ws = _vil_ws.get(key)
+        if ws is None:
+            n = _lib.load().esvit_vil_sc_ws_floats(B, nx, ny, nH)
+            if n <= 0:
+                raise ValueError("esvit_vil_sc_bwd: problem too large for the workspace")
+            ws = _vil_ws[key] = torch.empty(n, dtype=F32, device=q.device)
+        dq, dkv = torch.empty_like(q), torch.empty_like(kv)
+        dvec = torch.empty_like(lse)
+        dbias, dbias_g = torch.empty_like(bias), torch.empty_like(bias_g)
+        _lib.call("esvit_vil_sc_bwd", _p(q), _p(kv), _p(bias), _p(bias_g), _p(mode), _p(out), _p(g), _p(lse), _p(lse_g),
+                  _p(dvec), _p(ws), _p(dq), _p(dkv), _p(dbias), _p(dbias_g), B, nx, ny, nH, scale, _stream())
+        return dq, dkv, dbias, dbias_g, None, None, None, None, None, None
+
+
 # ------------------------------------------------------------------------------------------------------------
 # optimiser-side multi-tensor ops
 

@@ -244,6 +244,23 @@ int esvit_dwbn_bwd_apply(const void* dy, const void* z, const void* y, const flo
                          const double* sums, float* coef, void* dx, float* part, float* dw, int B, int H, int W, int Hp,
                          int Wp, int C, int train, void* stream);
 
+/* ---- Vision Longformer (layers/longformer2d.py Long2DSCSelfAttention, W = 7, one global token, head dim 32) --------
+ * Per image N = 1 + nx*ny token rows, row 0 the global token: q bf16 [B*N, C] (unscaled), kv bf16 [B*N, 2C] as [k|v],
+ * out / dout / dq bf16 [B*N, C], dkv bf16 [B*N, 2C]; C = 32 nH.  mode int32 [1] in device memory: 0 = all nine
+ * neighbour chunks, 1..8 = the own chunk and the reference's mode_dict chunk, -1 = the own chunk only; a value outside
+ * -1..8 is clamped into that range.  bias / dbias fp32 [nH, 49, 442] (column
+ * 0: local -> global, 1 + j*49 + r: key r of neighbour chunk j; columns of chunks the mode skips are not read and their
+ * gradient is 0); bias_g / dbias_g fp32 [nH, N] (the global row).  lse / dvec fp32 [B, nH, chunks, 49], lse_g fp32 [B,
+ * nH]; ws fp32 scratch of esvit_vil_sc_ws_floats(B, nx, ny, nH) elements.  dbias / dbias_g are written.  No
+ * floating-point atomics. */
+int esvit_vil_sc_ws_floats(int B, int nx, int ny, int nH);
+int esvit_vil_sc_fwd(const void* q, const void* kv, const float* bias, const float* bias_g, const int* mode, void* out,
+                     float* lse, float* lse_g, int B, int nx, int ny, int nH, float scale, void* stream);
+int esvit_vil_sc_bwd(const void* q, const void* kv, const float* bias, const float* bias_g, const int* mode,
+                     const void* out, const void* dout, const float* lse, const float* lse_g, float* dvec, float* ws,
+                     void* dq, void* dkv, float* dbias, float* dbias_g, int B, int nx, int ny, int nH, float scale,
+                     void* stream);
+
 /* ---- optimiser-side multi-tensor kernels (host arrays of device pointers) ----------------------------------
  * ema_multi: teacher = teacher*m + student*(1-m), bit-exact with main_esvit.py:587-590.
  * clip_multi: per-tensor L2 clip of utils.py:106-115; sumsq_ws double[n] workspace; norms fp32[n] or NULL. */
