@@ -31,7 +31,7 @@
 namespace wa {
 
 static bool make_geo(Geo& g, int B, int H, int W, int C, int nH, int ws, int shift) {
-  if (B <= 0 || C != nH * HD || (ws != 7 && ws != 14) || shift < 0 || shift >= ws) return false;
+  if (B <= 0 || H <= 0 || W <= 0 || nH <= 0 || C != nH * HD || (ws != 7 && ws != 14) || shift < 0 || shift >= ws) return false;
   g.B = B; g.H = H; g.W = W; g.C = C; g.nH = nH; g.shift = shift;
   g.Hp = (H + ws - 1) / ws * ws;
   g.Wp = (W + ws - 1) / ws * ws;

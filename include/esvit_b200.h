@@ -62,7 +62,7 @@ int esvit_patch_embed_bwd(const float* img, const float* w, const float* bias, c
  * Folds pad / roll / window_partition / rel-pos bias / -100 shift mask / softmax / PV / window_reverse / roll / crop.
  * qkv bf16 [B,H,W,3C] ([q|k|v][head][32]) is the qkv GEMM output including its bias; qkv_bias bf16 [3C] is what a
  * padded slot holds (the bias alone); bias_table fp32 [(2ws-1)^2, nH]; out bf16 [B,H,W,C]; lse fp32
- * [B*nWindows, nH, ws*ws].  ws in {7,14}; head_dim 32.
+ * [B*nWindows, nH, ws*ws].  ws in {7,14}; head_dim 32; B, H, W, nH >= 1 and 0 <= shift < ws (else status 1001).
  * bias_ws fp32 [nH*8192]: caller-owned scratch (ws 7: the rel-pos bias expanded to [nH][64][64]; ws 14 backward: the
  * lane-expanded bias-gradient accumulator [nH][27][6][32], cleared and folded into dbias_table inside the call).
  * bias_ready (ws 7): 1 = bias_ws already holds the expansion written by esvit_window_attn_expand_bias for this table
