@@ -255,100 +255,10 @@ def residual_add(x: Tensor, delta: Optional[Tensor], keep: Optional[Tensor],
 
 
 # ------------------------------------------------------------------------------------------------------------
-class PatchMergeLNFn(Function):
-    """x fp32 [B, H*W, C] -> LN(2x2 gather) bf16 [B, ceil(H/2)*ceil(W/2), 4C]."""
-
-    @staticmethod
-    def forward(ctx, x, gamma, beta, eps: float, H: int, W: int):
-        x, gamma, beta = _chk(x, F32, "x"), _chk(gamma, F32, "gamma"), _chk(beta, F32, "beta")
-        B, L, C = x.shape
-        assert L == H * W
-        Lo = ((H + 1) // 2) * ((W + 1) // 2)
-        y = torch.empty(B, Lo, 4 * C, dtype=BF16, device=x.device)
-        mean = torch.empty(B * Lo, dtype=F32, device=x.device)
-        rstd = torch.empty(B * Lo, dtype=F32, device=x.device)
-        _lib.call("esvit_patch_merge_ln_fwd", _p(x), _p(gamma), _p(beta), eps, _p(y), _p(mean), _p(rstd), B, H, W, C,
-                  _stream())
-        ctx.save_for_backward(x, mean, rstd, gamma)
-        ctx.hw = (H, W)
-        return y
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, g):
-        x, mean, rstd, gamma = ctx.saved_tensors
-        H, W = ctx.hw
-        B, L, C = x.shape
-        g = _chk(g, BF16, "g")
-        dx = torch.empty_like(x)
-        acc, first = _acc(("merge", gamma.data_ptr()), (2, gamma.numel()), x.device)
-        dgamma, dbeta = acc[0], acc[1]
-        _lib.call("esvit_patch_merge_ln_bwd", _p(g), _p(x), _p(mean), _p(rstd), _p(gamma), _p(dx), _p(dgamma),
-                  _p(dbeta), B, H, W, C, _stream())
-        return (dx, dgamma, dbeta, None, None, None) if first else (dx, None, None, None, None, None)
-
-
-class TokenMeanFn(Function):
-    """region fp32 [B, N, C] -> pooled [B, C]."""
-
-    @staticmethod
-    def forward(ctx, region):
-        region = _chk(region, F32, "region")
-        B, N, C = region.shape
-        pooled = torch.empty(B, C, dtype=F32, device=region.device)
-        _lib.call("esvit_token_mean_fwd", _p(region), _p(pooled), B, N, C, _stream())
-        ctx.shape = (B, N, C)
-        return pooled
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, g):
-        B, N, C = ctx.shape
-        g = _chk(g, F32, "g")
-        d = torch.empty(B, N, C, dtype=F32, device=g.device)
-        _lib.call("esvit_token_mean_bwd", _p(g), None, _p(d), B, N, C, _stream())
-        return d
-
-
-class PatchEmbedFn(Function):
-    """img fp32 [B,3,H,W] -> LN(conv4x4/4) fp32 [B, (H/4)(W/4), E]."""
-
-    @staticmethod
-    def forward(ctx, img, w, bias, gamma, beta, eps: float):
-        img, w, bias = _chk(img, F32, "img"), _chk(w, F32, "w"), _chk(bias, F32, "bias")
-        gamma, beta = _chk(gamma, F32, "gamma"), _chk(beta, F32, "beta")
-        B, Cin, H, W = img.shape
-        E = w.shape[0]
-        if Cin != 3 or tuple(w.shape[1:]) != (3, 4, 4):
-            raise ValueError("PatchEmbed kernel supports in_chans=3, patch_size=4")
-        T = B * (H // 4) * (W // 4)
-        out = torch.empty(B, (H // 4) * (W // 4), E, dtype=F32, device=img.device)
-        mean = torch.empty(T, dtype=F32, device=img.device)
-        rstd = torch.empty(T, dtype=F32, device=img.device)
-        _lib.call("esvit_patch_embed_fwd", _p(img), _p(w), _p(bias), _p(gamma), _p(beta), eps, _p(out), _p(mean),
-                  _p(rstd), B, H, W, E, _stream())
-        ctx.save_for_backward(img, w, bias, gamma, mean, rstd)
-        return out
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, g):
-        img, w, bias, gamma, mean, rstd = ctx.saved_tensors
-        B, _, H, W = img.shape
-        E = w.shape[0]
-        g = _chk(g, F32, "g")
-        dw, first = _acc(("pe_w", w.data_ptr()), tuple(w.shape), w.device)
-        acc, _ = _acc(("pe_b", w.data_ptr()), (3, E), w.device)
-        db, dgamma, dbeta = acc[0], acc[1], acc[2]
-        _lib.call("esvit_patch_embed_bwd", _p(img), _p(w), _p(bias), _p(gamma), _p(mean), _p(rstd), _p(g), _p(dw),
-                  _p(db), _p(dgamma), _p(dbeta), B, H, W, E, _stream())
-        return (None, dw, db, dgamma, dbeta, None) if first else (None, None, None, None, None, None)
-
-
 class PatchEmbedGroupsFn(Function):
-    """PatchEmbedFn over several resolution groups written into ONE token buffer fp32 [sum_g B_g L_g, E] (the
-    concatenated residual stream of the fused multi-crop forward): no torch.cat of the groups' outputs (267 MB copied
-    per step for Swin-T at B = 64) and no split of the gradient."""
+    """imgs fp32 [B_g, 3, H_g, W_g], one per resolution group -> LN(conv4x4/4) of every group written into ONE token
+    buffer fp32 [sum_g B_g (H_g/4)(W_g/4), E] (the concatenated residual stream of the Swin forward): no torch.cat of
+    the groups' outputs (267 MB copied per step for Swin-T at B = 64) and no split of the gradient."""
 
     @staticmethod
     def forward(ctx, w, bias, gamma, beta, eps: float, *imgs):
@@ -416,57 +326,15 @@ def cat_adjacent(ts):
 ATTN_WS_FLOATS = 8192  # per head; include/esvit_b200.h (expanded bias for ws 7, bias-gradient accumulator for ws 14)
 
 
-class WindowAttentionFn(Function):
-    """qkv bf16 [B, H*W, 3C] (qkv GEMM output incl. bias) -> attention output bf16 [B, H*W, C] in token order
-    (pad / roll / partition / reverse folded in).  qkv_bias (fp32 [3C] parameter) supplies the value of padded slots
-    and receives the COMPLETE qkv-bias gradient from the backward kernel (column sums of dq/dk/dv)."""
-
-    @staticmethod
-    def forward(ctx, qkv, qkv_bias, bias_table, H: int, W: int, num_heads: int, ws: int, shift: int, scale: float,
-                bias_exp: Optional[Tensor]):
-        qkv = _chk(qkv, BF16, "qkv")
-        qkv_bias = _chk(qkv_bias, F32, "qkv_bias")
-        bias_table = _chk(bias_table, F32, "relative_position_bias_table")
-        B, L, C3 = qkv.shape
-        C = C3 // 3
-        assert L == H * W
-        qb = shadow.lookup(qkv_bias)  # optimiser-maintained bf16 copy (no cast kernel per call) when registered
-        if qb is None:
-            qb = qkv_bias.detach().to(BF16)
-        nwin = B * (-(-H // ws)) * (-(-W // ws))
-        out = torch.empty(B, L, C, dtype=BF16, device=qkv.device)
-        lse = torch.empty(nwin * num_heads * ws * ws, dtype=F32, device=qkv.device)
-        # bias_exp: the table already expanded for this step by expand_rel_pos_bias (shared by every call and by the
-        # backward); without it each call expands into its own scratch
-        ready = 1 if (bias_exp is not None and ws == 7) else 0
-        bws = bias_exp if ready else torch.empty(num_heads * ATTN_WS_FLOATS, dtype=F32, device=qkv.device)
-        _lib.call("esvit_window_attn_fwd", _p(qkv), _p(qb), _p(bias_table), _p(bws), ready, _p(out), _p(lse), B, H, W, C,
-                  num_heads, ws, shift, scale, _stream())
-        ctx.save_for_backward(qkv, qb, bias_table, out, lse, bws if ready else None)
-        ctx.geo = (B, H, W, C, num_heads, ws, shift, scale)
-        return out
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, g):
-        qkv, qb, bias_table, out, lse, bias_exp = ctx.saved_tensors
-        B, H, W, C, nH, ws, shift, scale = ctx.geo
-        ready = 1 if bias_exp is not None else 0
-        g = _chk(g, BF16, "g")
-        dqkv = torch.empty_like(qkv)
-        dtable, first = _acc(("attn_t", bias_table.data_ptr()), tuple(bias_table.shape), qkv.device)
-        dqb, _ = _acc(("attn_b", bias_table.data_ptr()), (3 * C,), qkv.device)
-        bws = bias_exp if ready else torch.empty(nH * ATTN_WS_FLOATS, dtype=F32, device=qkv.device)
-        _lib.call("esvit_window_attn_bwd", _p(qkv), _p(qb), _p(bias_table), _p(bws), ready, _p(out), _p(g), _p(lse), _p(dqkv),
-                  _p(dtable), _p(dqb), B, H, W, C, nH, ws, shift, scale, _stream())
-        return dqkv, (dqb if first else None), (dtable if first else None), None, None, None, None, None, None, None
-
-
 class WindowAttentionGroupsFn(Function):
-    """WindowAttentionFn over several resolution groups stored back to back in ONE token-major tensor: qkv bf16
-    [T, 3C], group g = (B, H, W, row0) = rows [row0, row0 + B*H*W) holding B maps of H x W tokens.  One kernel launch
-    per group on pointer offsets (no slicing / concatenation copies); the table / qkv-bias gradients of all groups
-    accumulate into the same buffers."""
+    """Shifted-window attention over resolution groups stored back to back in ONE token-major tensor: qkv bf16 [T, 3C]
+    (qkv GEMM output incl. bias), group g = (B, H, W, row0) = rows [row0, row0 + B*H*W) holding B maps of H x W tokens
+    -> attention output bf16 [T, C] in token order (pad / roll / partition / reverse folded in).  One kernel launch per
+    group on pointer offsets (no slicing / concatenation copies).  qkv_bias (fp32 [3C] parameter) supplies the value of
+    padded slots and receives the COMPLETE qkv-bias gradient from the backward kernel (column sums of dq/dk/dv); the
+    table / qkv-bias gradients of all groups accumulate into the same buffers.  bias_exp: the table already expanded
+    for this step by expand_rel_pos_bias (shared by every call and by the backward), or None: each call expands into
+    its own scratch."""
 
     @staticmethod
     def forward(ctx, qkv, qkv_bias, bias_table, groups, num_heads: int, ws: int, shift: int, scale: float, bias_exp):
@@ -513,8 +381,9 @@ class WindowAttentionGroupsFn(Function):
 
 
 class PatchMergeLNGroupsFn(Function):
-    """PatchMergeLNFn over resolution groups stored back to back: x fp32 [T, C] -> bf16 [T', 4C] (T' = sum of
-    B * ceil(H/2) * ceil(W/2)), one launch per group on pointer offsets."""
+    """LN of the 2x2 gather of Swin's PatchMerging over resolution groups stored back to back: x fp32 [T, C] -> bf16
+    [T', 4C] (T' = sum of B * ceil(H/2) * ceil(W/2); odd maps are zero-padded), one launch per group on pointer
+    offsets."""
 
     @staticmethod
     def forward(ctx, x, gamma, beta, eps: float, groups):
@@ -551,7 +420,8 @@ class PatchMergeLNGroupsFn(Function):
 
 
 class TokenMeanGroupsFn(Function):
-    """TokenMeanFn over resolution groups stored back to back: region fp32 [T, C] -> pooled [sum B, C]."""
+    """Mean over the tokens of every sample of resolution groups stored back to back: region fp32 [T, C] -> pooled
+    fp32 [sum B, C]."""
 
     @staticmethod
     def forward(ctx, region, groups):
@@ -726,7 +596,8 @@ def _vit_split(x, cls, region, groups, direction):
 @torch.no_grad()
 def window_attention_probs(qkv: Tensor, qkv_bias: Tensor, bias_table: Tensor, H: int, W: int, num_heads: int, ws: int,
                            shift: int, scale: float, bias_exp: Optional[Tensor] = None) -> Tensor:
-    """The attention probabilities of the WindowAttentionFn call with the same arguments, fp32
+    """The attention probabilities of the WindowAttentionGroupsFn call on the one group (B, H, W, 0) of qkv bf16
+    [B, H*W, 3C] with the same other arguments, fp32
     [B*nWy*nWx, nH, ws*ws, ws*ws] in the reference's layout (the `attn` that WindowAttention.forward returns,
     models/swin_transformer.py:141-152): windows of the padded frame rolled by -shift, rows and columns of padded slots
     included.  Not differentiable."""
@@ -751,7 +622,7 @@ def window_attention_probs(qkv: Tensor, qkv_bias: Tensor, bias_table: Tensor, H:
 
 def expand_rel_pos_bias(bias_table: Tensor, num_heads: int, ws: int) -> Optional[Tensor]:
     """ws = 7: the rel-pos bias table expanded ONCE for all attention calls (both crop groups, forward and backward) that
-    use it this step -> fp32 [nH*4096] to pass as WindowAttentionFn's bias_exp; ws = 14: None (staged per CTA)."""
+    use it this step -> fp32 [nH*4096] to pass as WindowAttentionGroupsFn's bias_exp; ws = 14: None (staged per CTA)."""
     if ws != 7:
         return None
     bias_table = _chk(bias_table.detach(), F32, "relative_position_bias_table")

@@ -6,20 +6,23 @@ same parameter / buffer names (teacher.load_state_dict(student.state_dict()) and
 ``SwinTransformer.forward`` (models/swin_transformer.py:713-763).
 
 Execution model (what differs from the reference, see DESIGN.md):
-  * the residual stream is fp32 token-major [B, H*W, C]; every branch output is bf16;
+  * every entry point runs one path: the resolution groups of a call (one group per crop size; a plain batch is one
+    group) are stored back to back in ONE fp32 token-major residual stream [T, C], described by the geometry
+    grp = ((B, H, W, row0), ...); every per-token op runs once over all of them; every branch output is bf16;
   * ``x = shortcut + drop_path(branch)`` is fused with the NEXT LayerNorm (ops.add_layer_norm), so a block is
     LN -> qkv GEMM -> window-attention kernel -> proj GEMM -> add+LN -> fc1 GEMM -> GELU -> fc2 GEMM, with the
     trailing add deferred into the following block / PatchMerging / final norm;
   * pad, cyclic shift, window partition/reverse, the relative-position bias gather and the shift mask never
     exist as tensors - the attention kernel derives them from (H, W, window, shift);
-  * the plain GEMMs (qkv, proj, fc1, fc2, reduction) are bf16 library GEMMs (torch.nn.functional.linear).
+  * the plain GEMMs (qkv, proj, fc1, fc2, reduction) run on the wgmma GEMM family (esvit_b200.linear; library GEMMs
+    with ESVIT_GEMM2=0).
 """
 from __future__ import annotations
 
 import math
 import os
 from functools import partial
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, Optional, Sequence
 
 import torch
 import torch.nn as nn
@@ -33,10 +36,6 @@ BF16 = torch.bfloat16
 
 # fc1 + bias + GELU as one wgmma/TMA GEMM (esvit_gemm_bias_act) instead of library GEMM + GELU kernel
 USE_TCGEN05_FC1 = os.environ.get("ESVIT_TCGEN05_FC1", "1") != "0"
-# run every per-token op (GEMMs, add+LN, MLP) ONCE over the concatenated tokens of all resolution groups of a multi-crop
-# forward instead of once per group; attention / patch merging / pooling launch per group on slices of the same buffers
-# (SwinTransformer._forward_fused_groups).  ESVIT_FUSE_GROUPS=0 restores the reference's per-group loop.
-USE_FUSED_GROUPS = os.environ.get("ESVIT_FUSE_GROUPS", "1") != "0"
 # every Linear (forward, input gradient, weight gradient) on the wgmma GEMM family (esvit_b200.linear)
 # instead of library GEMMs; ESVIT_GEMM2=0 restores the library-GEMM path of round 1
 USE_GEMM2 = os.environ.get("ESVIT_GEMM2", "1") != "0"
@@ -57,19 +56,6 @@ class _CastCache:
 
     def __init__(self):
         self.d: Dict[int, Tensor] = {}
-        self.drop_plan = None  # [(block id, drop_prob)] of the backbone in execution order (set by the backbone)
-        self.keep_prob = None  # device fp32 [2*nblk, 1]: 1 - drop_prob per DropPath call
-        self.group = 0         # resolution group being run
-        self._drop = {}        # (group, batch size) -> {block id: (k1, k2)}
-
-    def drop_keeps(self, batch: int, drop_prob: float, device, key):
-        tab = self._drop.get((self.group, batch))
-        if tab is None:  # one draw for every block of this resolution group
-            r = torch.rand(len(self.drop_plan) * 2, batch, dtype=torch.float32, device=device)
-            keeps = r.add_(self.keep_prob).floor_().div_(self.keep_prob)      # timm: floor(keep_prob + U) / keep_prob
-            tab = self._drop[(self.group, batch)] = {bid: (keeps[2 * i], keeps[2 * i + 1])
-                                                     for i, (bid, _) in enumerate(self.drop_plan)}
-        return tab[key]
 
     def __call__(self, p: Optional[Tensor]) -> Optional[Tensor]:
         if p is None:
@@ -125,15 +111,11 @@ def drop_path_keep(batch: int, drop_prob: float, training: bool, device) -> Opti
     return r.floor_().div_(keep_prob)
 
 
-def drop_path_keeps(batch: int, drop_prob: float, training: bool, device, cc, key):
-    """The two DropPath scales of one block (attention branch, MLP branch).  Same distribution as drop_path_keep; the
-    uniforms of ALL blocks of one backbone pass are drawn by one torch.rand and turned into scales by two kernels
-    (registered in the pass' _CastCache) instead of four tiny kernels per DropPath call (~100 launches per step)."""
-    if drop_prob == 0. or not training:
-        return None, None
-    if cc is None or cc.drop_plan is None:
-        return (drop_path_keep(batch, drop_prob, training, device), drop_path_keep(batch, drop_prob, training, device))
-    return cc.drop_keeps(batch, drop_prob, device, key)
+def _one_group(x: Tensor):
+    """a [B, H*W, C] batch of square maps as the stream of one resolution group -> (x [B*H*W, C], grp)"""
+    B, L, C = x.shape
+    H = int(math.sqrt(L))
+    return x.reshape(B * L, C), ((B, H, H, 0),)
 
 
 class Mlp(nn.Module):
@@ -194,28 +176,22 @@ class WindowAttention(nn.Module):
         self.proj = nn.Linear(dim, dim)
         _trunc_normal_(self.relative_position_bias_table, std=.02)
 
-    def attend(self, y: Tensor, H: int, W: int, shift: int, cc: Optional[_CastCache] = None,
+    def attend(self, y: Tensor, grp, shift: int, cc: Optional[_CastCache] = None,
                maps: Optional[List[Tensor]] = None) -> Tensor:
-        """y = norm1(x) bf16 [B, H*W, C] in token order -> proj(attention) bf16 [B, H*W, C]; proj.bias gets its gradient
-        from the residual-add kernel the caller routes it through.  maps: a list to append the attention probabilities
-        to (ops.window_attention_probs, fp32 [B*nW, nH, N, N]), or None."""
-        qkv = _lin_c(y, self.qkv, cc)
-        ws = self.window_size[0]
-        bexp = None if cc is None else cc.expanded_bias(self.relative_position_bias_table, self.num_heads, ws)
-        a = ops.WindowAttentionFn.apply(qkv, self.qkv.bias, self.relative_position_bias_table, H, W, self.num_heads,
-                                        ws, shift, float(self.scale), bexp)
-        if maps is not None:
-            maps.append(ops.window_attention_probs(qkv, self.qkv.bias, self.relative_position_bias_table, H, W,
-                                                   self.num_heads, ws, shift, float(self.scale), bexp))
-        return _lin_c(a, self.proj, cc)
-
-    def attend_groups(self, y: Tensor, grp, shift: int, cc: Optional[_CastCache] = None) -> Tensor:
-        """attend() for the concatenated tokens [T, C] of several resolution groups grp = [(B, H, W, row0)]."""
+        """y = norm1(x) bf16 [T, C] in token order of the resolution groups grp = ((B, H, W, row0), ...) ->
+        proj(attention) bf16 [T, C]; proj.bias gets its gradient from the residual-add kernel the caller routes it
+        through.  maps: a list to append the attention probabilities to (ops.window_attention_probs, fp32
+        [B*nW, nH, N, N]; one group only), or None."""
         qkv = _lin_c(y, self.qkv, cc)
         ws = self.window_size[0]
         bexp = None if cc is None else cc.expanded_bias(self.relative_position_bias_table, self.num_heads, ws)
         a = ops.WindowAttentionGroupsFn.apply(qkv, self.qkv.bias, self.relative_position_bias_table, tuple(grp),
                                               self.num_heads, ws, shift, float(self.scale), bexp)
+        if maps is not None:
+            (B, H, W, _), = grp
+            maps.append(ops.window_attention_probs(qkv.view(B, H * W, -1), self.qkv.bias,
+                                                   self.relative_position_bias_table, H, W, self.num_heads, ws, shift,
+                                                   float(self.scale), bexp))
         return _lin_c(a, self.proj, cc)
 
     def forward(self, x: Tensor, mask: Optional[Tensor] = None):
@@ -227,7 +203,7 @@ class WindowAttention(nn.Module):
         ws = self.window_size[0]
         B_, N, C = x.shape
         assert N == ws * ws
-        return self.attend(x.to(BF16), ws, ws, 0), None
+        return self.attend(x.to(BF16).reshape(B_ * N, C), ((B_, ws, ws, 0),), 0).view(B_, N, C), None
 
 
 class SwinTransformerBlock(nn.Module):
@@ -247,35 +223,31 @@ class SwinTransformerBlock(nn.Module):
         self.norm2 = norm_layer(dim)
         self.mlp = Mlp(dim, int(dim * mlp_ratio), act_layer=act_layer, drop=drop)
 
-    def fused(self, x: Tensor, pending, cc: Optional[_CastCache] = None, maps: Optional[List[Tensor]] = None):
-        """(x fp32 [B,L,C], pending=(delta bf16, keep, delta_bias) or None) -> (x, pending): the MLP branch's
-        residual add (and fc2 bias) is deferred into the next fused add+LN.  maps: see WindowAttention.attend."""
+    def fused(self, x: Optional[Tensor], pending, grp, cc: Optional[_CastCache], k1: Optional[Tensor],
+              k2: Optional[Tensor], maps: Optional[List[Tensor]] = None):
+        """(x fp32 [T, C] of the resolution groups grp = ((B, H, W, row0), ...), pending = (delta bf16, keep,
+        delta_bias) or None) -> (x, pending): the MLP branch's residual add (and fc2 bias) is deferred into the next
+        fused add+LN.  x None: the stream starts as fp32(delta) (after PatchMerging).  k1 / k2: per-ROW DropPath
+        scales (fp32 [T]) or None.  maps: see WindowAttention.attend."""
         delta, keep, dbias = pending if pending is not None else (None, None, None)
-        B, L, C = (x if x is not None else delta).shape  # x None: the stream starts as fp32(delta) (after PatchMerging)
-        H = W = int(math.sqrt(L))
         x, y = ops.add_layer_norm(x, delta, keep, self.norm1.weight, self.norm1.bias, self.norm1.eps, delta_bias=dbias)
-        a = self.attn.attend(y, H, W, self.shift_size, cc, maps)
-        k1, k2 = drop_path_keeps(B, self.drop_prob, self.training, x.device, cc, id(self))
+        a = self.attn.attend(y, grp, self.shift_size, cc, maps)
         x, y = ops.add_layer_norm(x, a, k1, self.norm2.weight, self.norm2.bias, self.norm2.eps,
                                   delta_bias=self.attn.proj.bias)
         z = self.mlp.fused(y, cc)
         return x, (z, k2, self.mlp.fc2.bias)
 
-    def fused_groups(self, x: Optional[Tensor], pending, grp, cc, k1: Optional[Tensor], k2: Optional[Tensor]):
-        """fused() over the concatenated tokens x fp32 [T, C] of the resolution groups grp = [(B, H, W, row0)];
-        k1 / k2: per-ROW DropPath scales (fp32 [T]) or None."""
-        delta, keep, dbias = pending if pending is not None else (None, None, None)
-        x, y = ops.add_layer_norm(x, delta, keep, self.norm1.weight, self.norm1.bias, self.norm1.eps, delta_bias=dbias)
-        a = self.attn.attend_groups(y, grp, self.shift_size, cc)
-        x, y = ops.add_layer_norm(x, a, k1, self.norm2.weight, self.norm2.bias, self.norm2.eps,
-                                  delta_bias=self.attn.proj.bias)
-        z = self.mlp.fused(y, cc)
-        return x, (z, k2, self.mlp.fc2.bias)
+    def keeps(self, B: int, L: int, device) -> List[Optional[Tensor]]:
+        """[k1, k2]: the two DropPath scales of a call on B samples of L tokens outside the backbone, drawn per sample
+        (drop_path_keep) and spread per row (fp32 [B*L]); None = identity."""
+        ks = [drop_path_keep(B, self.drop_prob, self.training, device) for _ in range(2)]
+        return [None if k is None else k.repeat_interleave(L) for k in ks]
 
     def forward(self, x: Tensor):
         """Reference signature: x [B, L, C] -> (x, attn); attn probabilities are not materialised (None)."""
-        x, pend = self.fused(x.float(), None)
-        return ops.residual_add(x, *pend), None
+        xs, grp = _one_group(x.float())
+        xs, pend = self.fused(xs, None, grp, None, *self.keeps(x.shape[0], x.shape[1], x.device))
+        return ops.residual_add(xs, *pend).view(x.shape), None
 
 
 class PatchMerging(nn.Module):
@@ -285,23 +257,16 @@ class PatchMerging(nn.Module):
         self.reduction = nn.Linear(4 * dim, 2 * dim, bias=False)
         self.norm = norm_layer(4 * dim)
 
-    def forward(self, x: Tensor, cc: Optional[_CastCache] = None) -> Tensor:
-        """x fp32 [B, H*W, C] -> fp32 [B, H*W/4, 2C]."""
-        B, L, C = x.shape
-        H = W = int(math.sqrt(L))
-        return self.fused(x, cc).float()
+    def forward(self, x: Tensor) -> Tensor:
+        """x fp32 [B, H*W, C] -> fp32 [B, ceil(H/2)*ceil(W/2), 2C]."""
+        xs, grp = _one_group(x)
+        m, _ = self.fused(xs, grp)
+        return m.float().view(x.shape[0], -1, m.shape[-1])
 
-    def fused(self, x: Tensor, cc: Optional[_CastCache] = None) -> Tensor:
-        """-> bf16 [B, H*W/4, 2C]; the caller starts the next stage's fp32 residual stream from it inside the next
-        add+LN kernel (ops.add_layer_norm with x=None) instead of a separate cast pass."""
-        B, L, C = x.shape
-        H = W = int(math.sqrt(L))
-        y = ops.PatchMergeLNFn.apply(x, self.norm.weight, self.norm.bias, self.norm.eps, H, W)
-        return _lin_c(y, self.reduction, cc)
-
-
-    def fused_groups(self, x: Tensor, grp, cc: Optional[_CastCache] = None):
-        """fused() over concatenated groups: x fp32 [T, C] -> (bf16 [T', 2C], the groups' new geometry)."""
+    def fused(self, x: Tensor, grp, cc: Optional[_CastCache] = None):
+        """x fp32 [T, C] of the resolution groups grp = ((B, H, W, row0), ...) -> (bf16 [T', 2C], the groups' new
+        geometry); the caller starts the next stage's fp32 residual stream from it inside the next add+LN kernel
+        (ops.add_layer_norm with x=None) instead of a separate cast pass."""
         y = ops.PatchMergeLNGroupsFn.apply(x, self.norm.weight, self.norm.bias, self.norm.eps, tuple(grp))
         new_grp, row0 = [], 0
         for B, H, W, _ in grp:
@@ -325,56 +290,56 @@ class BasicLayer(nn.Module):
                                  norm_layer=norm_layer) for i in range(depth)])
         self.downsample = downsample(input_resolution, dim=dim, norm_layer=norm_layer) if downsample else None
 
-    def fused(self, x: Optional[Tensor], cc: Optional[_CastCache] = None, pend=None,
-              maps: Optional[List[Tensor]] = None):
-        """(x fp32 or None, pend) -> (x, pend).  After a downsample the stream is handed on as (None, (merged bf16, None,
-        None)): the next stage's first add+LN turns it into the fp32 residual.  maps: a list to append every block's
-        attention probabilities to, or None."""
-        for blk in self.blocks:
-            x, pend = blk.fused(x, pend, cc, maps)
-        if self.downsample is not None:
-            x = ops.residual_add(x, *pend)
-            return None, (self.downsample.fused(x, cc), None, None)
-        return x, pend
-
-    def fused_groups(self, x: Optional[Tensor], pend, grp, cc, keeps: Optional[Tensor]):
-        """fused() over concatenated groups; keeps: per-row DropPath scales fp32 [2*depth, T] of this layer or None."""
-        for i, blk in enumerate(self.blocks):
+    def fused(self, x: Optional[Tensor], pend, grp, cc: Optional[_CastCache], keeps: Optional[Sequence[Tensor]],
+              maps: Optional[Sequence[Optional[List[Tensor]]]] = None, taps=None):
+        """(x fp32 [T, C] or None, pend) over the resolution groups grp = ((B, H, W, row0), ...) -> (x, pend, grp after
+        the downsample).  After a downsample the stream is handed on as (None, (merged bf16, None, None)): the next
+        stage's first add+LN turns it into the fp32 residual.  keeps: per-row DropPath scales [2*depth][T] of this
+        layer or None.  Per block j: maps[j] is the list its attention probabilities are appended to, or None;
+        taps[j], if not None, makes the block's output materialise (residual_add) and is called with it and grp, and
+        the stream continues from it."""
+        for j, blk in enumerate(self.blocks):
             k1 = k2 = None
             if keeps is not None and blk.drop_prob > 0. and blk.training:
-                k1, k2 = keeps[2 * i], keeps[2 * i + 1]
-            x, pend = blk.fused_groups(x, pend, grp, cc, k1, k2)
+                k1, k2 = keeps[2 * j], keeps[2 * j + 1]
+            x, pend = blk.fused(x, pend, grp, cc, k1, k2, None if maps is None else maps[j])
+            if taps is not None and taps[j] is not None:
+                x, pend = ops.residual_add(x, *pend), None
+                taps[j](x, grp)
         if self.downsample is not None:
-            x = ops.residual_add(x, *pend)
-            m, grp = self.downsample.fused_groups(x, grp, cc)
+            if pend is not None:
+                x = ops.residual_add(x, *pend)
+            m, grp = self.downsample.fused(x, grp, cc)
             return None, (m, None, None), grp
         return x, pend, grp
 
+    def _forward(self, x: Tensor, maps=None, taps=None) -> Tensor:
+        """x [B, L, C] as one group through fused() -> fp32 [B, L', C'] after the downsample"""
+        B, L, _ = x.shape
+        keeps = [k for blk in self.blocks for k in blk.keeps(B, L, x.device)]
+        xs, grp = _one_group(x.float())
+        xs, pend, _ = self.fused(xs, None, grp, None, keeps, maps, taps)
+        if xs is None:  # after the downsample: the merged bf16 tokens
+            xs = pend[0].float()
+        elif pend is not None:
+            xs = ops.residual_add(xs, *pend)
+        return xs.view(B, -1, xs.shape[-1])
+
     def forward(self, x: Tensor) -> Tensor:
-        return self._forward(x, None)
+        return self._forward(x)
 
     def forward_with_attention(self, x: Tensor):
         """models/swin_transformer.py:492-499: x [B, L, C] -> (x after the downsample, [attention probabilities of
         every block, fp32 [B*nW, nH, N, N]]).  The probabilities do not require grad."""
         maps = []
-        return self._forward(x, maps), maps
-
-    def _forward(self, x: Tensor, maps: Optional[List[Tensor]]) -> Tensor:
-        x, pend = self.fused(x.float(), maps=maps)
-        if x is None:
-            return pend[0].float()
-        return x if pend is None else ops.residual_add(x, *pend)
+        return self._forward(x, maps=[maps] * len(self.blocks)), maps
 
     def forward_with_features(self, x: Tensor):
         """models/swin_transformer.py:483-490: x [B, L, C] -> (x after the downsample, [output of every block]), fp32."""
-        x, fea = x.float(), []
-        for blk in self.blocks:
-            x, pend = blk.fused(x, None)
-            x = ops.residual_add(x, *pend)
-            fea.append(x)
-        if self.downsample is not None:
-            x = self.downsample(x)
-        return x, fea
+        B, L, _ = x.shape
+        fea = []
+        y = self._forward(x, taps=[lambda xs, grp: fea.append(xs.view(B, L, -1))] * len(self.blocks))
+        return y, fea
 
 
 class PatchEmbed(nn.Module):
@@ -391,10 +356,22 @@ class PatchEmbed(nn.Module):
         self.proj = nn.Conv2d(in_chans, embed_dim, kernel_size=patch_size, stride=patch_size)  # parameter container
         self.norm = norm_layer(embed_dim)
 
+    def fused(self, imgs: Sequence[Tensor]):
+        """fp32 crops, one [B_g, 3, S_g, S_g] tensor per resolution group -> (the residual stream fp32 [T, E] with the
+        groups back to back, grp = ((B, H, W, row0), ...))."""
+        grp, row0 = [], 0
+        for im in imgs:
+            B, H, W = im.shape[0], im.shape[2] // 4, im.shape[3] // 4
+            grp.append((B, H, W, row0))
+            row0 += B * H * W
+        x = ops.PatchEmbedGroupsFn.apply(self.proj.weight, self.proj.bias, self.norm.weight, self.norm.bias,
+                                         self.norm.eps, *imgs)
+        return x, grp
+
     def forward(self, x: Tensor) -> Tensor:
         """x fp32 [B,3,H,W] -> fp32 [B, (H/4)(W/4), E]."""
-        return ops.PatchEmbedFn.apply(x.float(), self.proj.weight, self.proj.bias, self.norm.weight, self.norm.bias,
-                                      self.norm.eps)
+        xs, _ = self.fused([x.float()])
+        return xs.view(x.shape[0], -1, xs.shape[-1])
 
 
 class SwinTransformer(nn.Module):
@@ -424,7 +401,7 @@ class SwinTransformer(nn.Module):
                 drop_path=dpr[sum(depths[:i]):sum(depths[:i + 1])], norm_layer=norm_layer,
                 downsample=PatchMerging if i < self.num_layers - 1 else None))
         self.norm = norm_layer(self.num_features)
-        self.avgpool = nn.AdaptiveAvgPool1d(1)  # structural parity only; ops.TokenMeanFn does the work
+        self.avgpool = nn.AdaptiveAvgPool1d(1)  # structural parity only; ops.TokenMeanGroupsFn does the work
         self.head = nn.Linear(self.num_features, num_classes) if num_classes > 0 else nn.Identity()
         self.use_dense_prediction = use_dense_prediction
         if self.use_dense_prediction:
@@ -448,67 +425,20 @@ class SwinTransformer(nn.Module):
     def no_weight_decay_keywords(self):
         return {'relative_position_bias_table'}
 
-    def forward_features(self, x: Tensor, cc: Optional[_CastCache] = None):
-        """models/swin_transformer.py:678-694 -> pooled fp32 [B, D] (and region fp32 [B, N, D] in dense mode)."""
-        x = self.patch_embed(x)
-        pend = None
-        for layer in self.layers:
-            x, pend = layer.fused(x, cc, pend)
-        delta, keep, dbias = pend if pend is not None else (None, None, None)
-        _, x_region = ops.add_layer_norm(x, delta, keep, self.norm.weight, self.norm.bias, self.norm.eps,
-                                         y_bf16=False, delta_bias=dbias)
-        pooled = ops.TokenMeanFn.apply(x_region)
-        if self.use_dense_prediction:
-            return pooled, x_region
-        return pooled
-
     def _row_samples(self, grp, device) -> Tensor:
         """int64 [T]: the (global) sample index of every token row of the concatenated groups (cached per geometry)."""
         cache = self.__dict__.setdefault("_rs_cache", {})
         key = (tuple(grp), device)
         t = cache.get(key)
         if t is None:
+            if len(cache) >= 32:  # a handful of crop geometries per run; keep the cache from growing with odd batches
+                cache.clear()
             parts, b0 = [], 0
             for B, H, W, _ in grp:
                 parts.append(torch.arange(b0, b0 + B, device=device).repeat_interleave(H * W))
                 b0 += B
             t = cache[key] = torch.cat(parts)
         return t
-
-    def _forward_fused_groups(self, x, groups, cc):
-        """Multi-crop forward with ONE pass over the concatenated tokens of all resolution groups for every per-token op
-        (same math and output order as the per-group loop of models/swin_transformer.py:713-763)."""
-        imgs, grp, row0 = [], [], 0
-        for s, e in groups:
-            im = ops.cat_adjacent(x[s:e]).float()
-            B, H, W = im.shape[0], im.shape[2] // 4, im.shape[3] // 4
-            imgs.append(im)
-            grp.append((B, H, W, row0))
-            row0 += B * H * W
-        pe = self.patch_embed
-        # every group's tokens straight into the concatenated stream (fp32 [T, E]); same kernels as PatchEmbed.forward
-        xa = ops.PatchEmbedGroupsFn.apply(pe.proj.weight, pe.proj.bias, pe.norm.weight, pe.norm.bias, pe.norm.eps, *imgs)
-        dev = xa.device
-        keeps_all = None
-        if self.training and any(blk.drop_prob > 0. for layer in self.layers for blk in layer.blocks):
-            kp = self._keep_prob_column(dev)                                    # [2*nblk, 1]
-            r = torch.rand(kp.shape[0], sum(g[0] for g in grp), dtype=torch.float32, device=dev)
-            keeps_all = r.add_(kp).floor_().div_(kp)                            # timm DropPath scale per (call, sample)
-        pend, off = None, 0
-        for layer in self.layers:
-            depth = len(layer.blocks)
-            keeps = None
-            if keeps_all is not None:
-                keeps = keeps_all[2 * off:2 * (off + depth)].index_select(1, self._row_samples(grp, dev))
-            xa, pend, grp = layer.fused_groups(xa, pend, grp, cc, keeps)
-            off += depth
-        delta, keep, dbias = pend if pend is not None else (None, None, None)
-        _, x_region = ops.add_layer_norm(xa, delta, keep, self.norm.weight, self.norm.bias, self.norm.eps,
-                                         y_bf16=False, delta_bias=dbias)
-        pooled = ops.TokenMeanGroupsFn.apply(x_region, tuple(grp))
-        if self.use_dense_prediction:
-            return self.head(pooled), self.head_dense(x_region), x_region, [H * W for _, H, W, _ in grp]
-        return self.head(pooled)
 
     def _keep_prob_column(self, device) -> Tensor:
         """device fp32 [2*nblk, 1] of 1 - drop_prob (two DropPath calls per block), built once per device."""
@@ -519,13 +449,53 @@ class SwinTransformer(nn.Module):
             t = cache[device] = torch.tensor(probs, dtype=torch.float32).to(device)
         return t
 
+    def _run(self, x, taps=None, maps=None):
+        """The backbone with ONE pass over the concatenated tokens of all resolution groups for every per-token op (same
+        math and output order as the per-group loop of models/swin_transformer.py:713-763).  x: fp32 crops, one
+        [B_g, 3, S_g, S_g] tensor per group, or patch-embedded tokens fp32 [B, L, C] (one group) -> (stream fp32 [T, C]
+        or None, pending (delta, keep, delta_bias) or None, the last stage's grp = ((B, H, W, row0), ...)).
+        taps / maps: None or one entry per block in execution order, see BasicLayer.fused."""
+        cc = _CastCache()
+        x, grp = _one_group(x) if isinstance(x, Tensor) else self.patch_embed.fused(x)
+        dev = x.device
+        keeps_all = None
+        if self.training and any(blk.drop_prob > 0. for layer in self.layers for blk in layer.blocks):
+            kp = self._keep_prob_column(dev)                                    # [2*nblk, 1]
+            r = torch.rand(kp.shape[0], sum(g[0] for g in grp), dtype=torch.float32, device=dev)
+            keeps_all = r.add_(kp).floor_().div_(kp)                            # timm DropPath scale per (call, sample)
+        pend, b = None, 0
+        for layer in self.layers:
+            d = len(layer.blocks)
+            keeps = None
+            if keeps_all is not None:
+                keeps = keeps_all[2 * b:2 * (b + d)].index_select(1, self._row_samples(grp, dev))
+            x, pend, grp = layer.fused(x, pend, grp, cc, keeps, None if maps is None else maps[b:b + d],
+                                       None if taps is None else taps[b:b + d])
+            b += d
+        return x, pend, grp
+
+    def _features(self, imgs: List[Tensor], taps=None):
+        """-> (pooled fp32 [sum B, D], region fp32 [T, D] = the final norm's tokens, the last stage's grp)"""
+        x, pend, grp = self._run(imgs, taps)
+        delta, keep, dbias = pend if pend is not None else (None, None, None)
+        _, region = ops.add_layer_norm(x, delta, keep, self.norm.weight, self.norm.bias, self.norm.eps,
+                                       y_bf16=False, delta_bias=dbias)
+        return ops.TokenMeanGroupsFn.apply(region, tuple(grp)), region, grp
+
+    def forward_features(self, x: Tensor):
+        """models/swin_transformer.py:678-694 -> pooled fp32 [B, D] (and region fp32 [B, N, D] in dense mode)."""
+        pooled, region, _ = self._features([x.float()])
+        if self.use_dense_prediction:
+            return pooled, region.view(x.shape[0], -1, region.shape[-1])
+        return pooled
+
     def forward_return_n_last_blocks(self, x: Tensor, n: int = 1, return_patch_avgpool: bool = False, depth=[]):
         """models/swin_transformer.py:799-837 (eval_linear.py's probe features): fp32 [B, sum C_i], the token means of
         the outputs of the last n blocks in execution order; outputs of last-stage blocks go through the final norm
         first.  return_patch_avgpool is ignored, as in the reference.  `depth` must equal the model's depths.
 
-        Runs the fused path of forward_features: only a tapped block's output is materialised (residual_add), and the
-        stream continues from it; the last block's normed output is the final add+LN output itself."""
+        Only a tapped block's output is materialised (residual_add), and the stream continues from it; the last
+        block's normed output is the final add+LN output itself."""
         depths = [len(layer.blocks) for layer in self.layers]
         if [int(d) for d in depth] != depths:
             raise ValueError(f"depth {list(depth)} does not match the model's depths {depths}")
@@ -533,27 +503,26 @@ class SwinTransformer(nn.Module):
         if not 1 <= int(n) <= total:
             raise ValueError(f"n must be in [1, {total}], got {n}")
         start, last = total - int(n), len(self.layers) - 1
-        cc = _CastCache()
-        x = self.patch_embed(x)
-        pend, out, b = None, [], 0
-        for i, layer in enumerate(self.layers):
-            for j, blk in enumerate(layer.blocks):
-                x, pend = blk.fused(x, pend, cc)
-                if b >= start and not (i == last and j == len(layer.blocks) - 1):
-                    x, pend = ops.residual_add(x, *pend), None
-                    y = ops.LayerNormFn.apply(x, self.norm.weight, self.norm.bias, self.norm.eps, False) if i == last else x
-                    out.append(ops.TokenMeanFn.apply(y))
-                b += 1
-            if layer.downsample is not None:
-                if pend is not None:
-                    x = ops.residual_add(x, *pend)
-                x, pend = None, (layer.downsample.fused(x, cc), None, None)
-        delta, keep, dbias = pend if pend is not None else (None, None, None)
-        _, x_region = ops.add_layer_norm(x, delta, keep, self.norm.weight, self.norm.bias, self.norm.eps,
-                                         y_bf16=False, delta_bias=dbias)
-        out.append(ops.TokenMeanFn.apply(x_region))
-        return torch.cat(out, dim=-1)
+        out = []
 
+        def tap(normed: bool, x: Tensor, grp):
+            y = ops.LayerNormFn.apply(x, self.norm.weight, self.norm.bias, self.norm.eps, False) if normed else x
+            out.append(ops.TokenMeanGroupsFn.apply(y, tuple(grp)))
+
+        taps = [partial(tap, i == last) for i, d in enumerate(depths) for _ in range(d)]
+        taps = [t if start <= b < total - 1 else None for b, t in enumerate(taps)]
+        pooled, _, _ = self._features([x.float()], taps)
+        return torch.cat(out + [pooled], dim=-1)
+
+    def _attention_maps(self, x, last: bool):
+        """_run's input -> the last block's attention probabilities (last) or every block's in execution order; only
+        the blocks asked for compute them."""
+        nblk = sum(len(layer.blocks) for layer in self.layers)
+        maps = []
+        self._run(x, maps=[None] * (nblk - 1) + [maps] if last else [maps] * nblk)
+        return maps[0] if last else maps
+
+    @torch.no_grad()
     def forward_selfattention(self, x: Tensor, n: int = 1):
         """models/swin_transformer.py:766-778 (analyze_models.py's attention maps): images fp32 [B, 3, S, S] -> the last
         block's attention probabilities if n == 1, else the list of every block's in execution order.  Each is fp32
@@ -561,10 +530,7 @@ class SwinTransformer(nn.Module):
         the padded, rolled map; rows and columns of padded slots are included."""
         if x.dim() != 4 or x.shape[2] != x.shape[3] or x.shape[2] % 4 != 0:
             raise ValueError(f"expected square images [B, 3, S, S] with S a multiple of 4, got {tuple(x.shape)}")
-        x = self.patch_embed(x)
-        if n == 1:
-            return self.forward_last_selfattention(x)
-        return self.forward_all_selfattention(x)
+        return self._attention_maps([x.float()], n == 1)
 
     def _check_tokens(self, x: Tensor) -> Tensor:
         side = math.isqrt(x.shape[1]) if x.dim() == 3 else 0
@@ -574,24 +540,14 @@ class SwinTransformer(nn.Module):
 
     @torch.no_grad()
     def forward_last_selfattention(self, x: Tensor) -> Tensor:
-        """models/swin_transformer.py:780-787: patch-embedded tokens [B, L, C] -> the last block's probabilities.  Runs the
-        fused path of forward_features; only the last block computes its probabilities."""
-        x, pend, cc, maps = self._check_tokens(x), None, _CastCache(), []
-        for layer in self.layers[:-1]:
-            x, pend = layer.fused(x, cc, pend)
-        blocks = self.layers[-1].blocks
-        for i, blk in enumerate(blocks):
-            x, pend = blk.fused(x, pend, cc, maps if i == len(blocks) - 1 else None)
-        return maps[0]
+        """models/swin_transformer.py:780-787: patch-embedded tokens [B, L, C] -> the last block's probabilities."""
+        return self._attention_maps(self._check_tokens(x), True)
 
     @torch.no_grad()
     def forward_all_selfattention(self, x: Tensor) -> List[Tensor]:
         """models/swin_transformer.py:789-796: patch-embedded tokens [B, L, C] -> every block's probabilities in execution
         order (sum(depths) tensors)."""
-        x, pend, cc, maps = self._check_tokens(x), None, _CastCache(), []
-        for layer in self.layers:
-            x, pend = layer.fused(x, cc, pend, maps)
-        return maps
+        return self._attention_maps(self._check_tokens(x), False)
 
     def forward_feature_maps(self, x: Tensor):
         d = self.use_dense_prediction
@@ -602,38 +558,19 @@ class SwinTransformer(nn.Module):
             self.use_dense_prediction = d
 
     def forward(self, x):
-        """Multi-crop forward (models/swin_transformer.py:713-763): consecutive same-resolution crops are
-        concatenated on the batch axis and run once; outputs are concatenated crop-major."""
+        """Multi-crop forward (models/swin_transformer.py:713-763): consecutive same-resolution crops form one group; the
+        outputs are concatenated group-major exactly as the reference's per-group loop concatenates them."""
         if not isinstance(x, list):
             x = [x]
-        cc = _CastCache()
-        if self.training:
-            cc.drop_plan = [(id(blk), blk.drop_prob) for layer in self.layers for blk in layer.blocks]
-            cc.keep_prob = self._keep_prob_column(x[0].device)
         groups, start = [], 0
         for i in range(1, len(x) + 1):
             if i == len(x) or x[i].shape[-1] != x[start].shape[-1]:
                 groups.append((start, i))
                 start = i
-        if USE_FUSED_GROUPS:
-            return self._forward_fused_groups(x, groups, cc)
+        pooled, region, grp = self._features([ops.cat_adjacent(x[s:e]).float() for s, e in groups])
         if self.use_dense_prediction:
-            cls_l, fea_l, npatch = [], [], []
-            for gi, (s, e) in enumerate(groups):
-                cc.group = gi
-                pooled, region = self.forward_features(ops.cat_adjacent(x[s:e]), cc)
-                B, N, C = region.shape
-                cls_l.append(pooled)
-                fea_l.append(region.reshape(B * N, C))
-                npatch.append(N)
-            output_cls = torch.cat(cls_l) if len(cls_l) > 1 else cls_l[0]
-            output_fea = torch.cat(fea_l) if len(fea_l) > 1 else fea_l[0]
-            return self.head(output_cls), self.head_dense(output_fea), output_fea, npatch
-        outs = []
-        for gi, (s, e) in enumerate(groups):
-            cc.group = gi
-            outs.append(self.forward_features(torch.cat(x[s:e]) if e - s > 1 else x[s], cc))
-        return self.head(torch.cat(outs) if len(outs) > 1 else outs[0])
+            return self.head(pooled), self.head_dense(region), region, [H * W for _, H, W, _ in grp]
+        return self.head(pooled)
 
 
 def get_cls_model(config, is_teacher=False, use_dense_prediction=False, **kwargs):

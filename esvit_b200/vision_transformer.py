@@ -271,7 +271,7 @@ class VisionTransformer(nn.Module):
 
     def _keeps(self, grp, device) -> Optional[Tensor]:
         """per-row DropPath scales fp32 [2*depth, T] (timm: floor(keep_prob + U) / keep_prob per (call, sample)), drawn
-        by one torch.rand as SwinTransformer._forward_fused_groups does; None when no block drops."""
+        by one torch.rand as SwinTransformer._run does; None when no block drops."""
         if not self.training or not any(blk.drop_prob > 0. for blk in self.blocks):
             return None
         cache = self.__dict__.setdefault("_kp_cache", {})
@@ -363,7 +363,7 @@ class VisionTransformer(nn.Module):
                 out.append(cls)
         if return_patch_avgpool:
             B, N = tg[0]
-            out.append(ops.TokenMeanFn.apply(region.view(B, N, -1)))
+            out.append(ops.TokenMeanGroupsFn.apply(region, ((B, 1, N, 0),)))
         return torch.cat(out, dim=-1)
 
     def forward_selfattention(self, x, n=1):

@@ -1,7 +1,7 @@
 """Host-side autograd plumbing of the module mirror, exercised WITHOUT a GPU: every C-ABI call is replaced by a no-op
 (outputs stay uninitialised), so only the wiring is checked - fused pending residuals, the x-less add+LN after
-PatchMerging, the per-pass DropPath plan, the shared gradient accumulators of the two crop groups, MlpFn.  The numerics
-of the same paths are the -m gpu tests."""
+PatchMerging, the per-row DropPath scales, the one-group standalone entry points, the shared gradient accumulators of
+the two crop groups, MlpFn.  The numerics of the same paths are the -m gpu tests."""
 import torch
 
 from esvit_b200 import _lib, engine, ops
@@ -28,22 +28,17 @@ def _patch(monkeypatch):
 import pytest
 
 
-@pytest.mark.parametrize("fuse_groups", [False, True])
-def test_every_parameter_gets_one_gradient(monkeypatch, fuse_groups):
-    from esvit_b200 import swin_transformer
-    _patch(monkeypatch)
-    monkeypatch.setattr(swin_transformer, "USE_FUSED_GROUPS", fuse_groups)
+def _swin(dense: bool):
+    """Swin-T W7 (drop_path_rate 0.1) with depths [1, 1, 2, 1] and its DINO head(s), in train mode"""
     spec = dict(engine.SWIN_SPECS["swin_tiny_w7"])
     spec["depths"] = [1, 1, 2, 1]
     torch.manual_seed(0)
-    net = engine.build_network(spec, 256, True, False, True, 224, None)
-    net.train()
-    B = 2
-    crops = [torch.randn(B, 3, 224, 224) for _ in range(2)] + [torch.randn(B, 3, 96, 96) for _ in range(3)]
-    cls, region, fea, npatch = net(crops)
-    assert cls.shape == (5 * B, 256) and npatch == [49, 9]
-    assert region.shape == (B * (2 * 49 + 3 * 9), 256) and fea.shape == (B * (2 * 49 + 3 * 9), 768)
-    loss = (cls.float() ** 2).sum() + (region.float() ** 2).sum()
+    net = engine.build_network(spec, 256, dense, False, True, 224, None)
+    return net.train()
+
+
+def _backward_gives_one_gradient_each(params, loss):
+    """loss.backward() inside a step: every parameter that requires grad gets exactly one fp32 gradient of its shape"""
     ops.begin_step("cpu", 1 << 22)
     try:
         loss.backward()
@@ -51,12 +46,67 @@ def test_every_parameter_gets_one_gradient(monkeypatch, fuse_groups):
     finally:
         ops.end_step()
     assert ops._Arena.accs is None
-    assert n_shared > 20  # LN / bias / rel-pos-table accumulators (shared by the two crop groups when run per group)
-    missing = [n for n, p in net.named_parameters() if p.requires_grad and p.grad is None]
+    missing = [n for n, p in params if p.requires_grad and p.grad is None]
     assert not missing, missing
-    for n, p in net.named_parameters():
+    for n, p in params:
         if p.grad is not None:
             assert p.grad.shape == p.shape and p.grad.dtype == torch.float32, n
+    return n_shared
+
+
+@pytest.mark.parametrize("dense", [True, False], ids=["dense", "view"])
+def test_every_parameter_gets_one_gradient(monkeypatch, dense):
+    _patch(monkeypatch)
+    net = _swin(dense)
+    B = 2
+    crops = [torch.randn(B, 3, 224, 224) for _ in range(2)] + [torch.randn(B, 3, 96, 96) for _ in range(3)]
+    if dense:
+        cls, region, fea, npatch = net(crops)
+        assert npatch == [49, 9]
+        assert region.shape == (B * (2 * 49 + 3 * 9), 256) and fea.shape == (B * (2 * 49 + 3 * 9), 768)
+        loss = (cls.float() ** 2).sum() + (region.float() ** 2).sum()
+    else:
+        cls = net(crops)
+        loss = (cls.float() ** 2).sum()
+    assert cls.shape == (5 * B, 256)
+    n_shared = _backward_gives_one_gradient_each(list(net.named_parameters()), loss)
+    assert n_shared > 20  # LN / bias / rel-pos-table accumulators
+
+
+def test_standalone_entry_points_wiring(monkeypatch):
+    """The entry points outside the multi-crop forward run the same resolution-group path on one group: shapes, and
+    the gradients of forward_features (train mode, DropPath, dense) and of a standalone block."""
+    _patch(monkeypatch)
+    net = _swin(True)
+    B = 2
+    pooled, region = net.forward_features(torch.randn(B, 3, 224, 224))
+    assert pooled.shape == (B, 768) and region.shape == (B, 49, 768)
+    backbone = [(n, p) for n, p in net.named_parameters() if not n.startswith("head")]
+    _backward_gives_one_gradient_each(backbone, (pooled ** 2).sum() + (region ** 2).sum())
+
+    net.eval()
+    x = torch.randn(B, 3, 224, 224)
+    for n, width in ((1, 768), (2, 384 + 768), (5, 96 + 192 + 384 + 384 + 768)):
+        assert net.forward_return_n_last_blocks(x, n, False, [1, 1, 2, 1]).shape == (B, width)
+    last = net.forward_selfattention(x, 1)
+    assert last.shape == (B, 24, 49, 49) and not last.requires_grad
+    maps = net.forward_selfattention(x, 2)
+    assert [tuple(m.shape) for m in maps] == [(B * 64, 3, 49, 49), (B * 16, 6, 49, 49), (B * 4, 12, 49, 49),
+                                              (B * 4, 12, 49, 49), (B, 24, 49, 49)]
+
+    layer, xs = net.layers[2], torch.randn(B, 14 * 14, 384)
+    y, fea = layer.forward_with_features(xs)
+    assert y.shape == (B, 49, 768) and [tuple(f.shape) for f in fea] == [(B, 196, 384)] * 2
+    y, maps = layer.forward_with_attention(xs)
+    assert y.shape == (B, 49, 768) and [tuple(m.shape) for m in maps] == [(B * 4, 12, 49, 49)] * 2
+
+    blk = layer.blocks[1].train()
+    assert blk.shift_size == 3 and blk.drop_prob > 0
+    xs.requires_grad_(True)
+    y, attn = blk(xs)
+    assert y.shape == xs.shape and y.dtype == torch.float32 and attn is None
+    _backward_gives_one_gradient_each(list(blk.named_parameters()), (y ** 2).sum())
+    assert xs.grad.shape == xs.shape
 
 
 def test_accumulators_are_private_outside_a_step(monkeypatch):
@@ -85,7 +135,7 @@ def test_group_geometry_of_the_concatenated_layout():
     assert net._row_samples(grp, torch.device("cpu")) is rs  # cached per geometry
     merged = []
     row0 = 0
-    for B, H, W, _ in grp:  # what PatchMerging.fused_groups hands to the next stage
+    for B, H, W, _ in grp:  # what PatchMerging.fused hands to the next stage
         merged.append((B, (H + 1) // 2, (W + 1) // 2, row0))
         row0 += B * ((H + 1) // 2) * ((W + 1) // 2)
     assert merged == [(2, 28, 28, 0), (3, 12, 12, 2 * 28 * 28)]

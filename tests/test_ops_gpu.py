@@ -63,47 +63,56 @@ def test_add_layer_norm(C, out_bf16):
 
 
 @pytest.mark.parametrize("H,C", [(8, 32), (6, 96), (7, 64), (14, 192), (4, 512)])
-def test_patch_merge_ln(H, C):
+def test_patch_merge_ln_groups(H, C):
+    """two resolution groups back to back (B = 2 maps of H x H, then 1 map of (H+1) x (H+1)), so the row offsets of
+    the second group and the odd / even padding are covered in one call"""
     from esvit_b200 import ops
     from oracle import swin as O
     torch.manual_seed(H * C)
-    B = 2
-    x = torch.randn(B, H * H, C)
+    sizes = ((2, H), (1, H + 1))
+    xs = [torch.randn(B, S * S, C) for B, S in sizes]
     g, b = 1 + 0.1 * torch.randn(4 * C), 0.1 * torch.randn(4 * C)
     W = torch.eye(4 * C)  # identity "reduction" so the oracle's gather+LN is observable
     sd = {"m.norm.weight": g.clone().requires_grad_(True), "m.norm.bias": b.clone().requires_grad_(True),
           "m.reduction.weight": W}
-    xr = x.clone().requires_grad_(True)
-    y_r = O.patch_merging(xr, sd, "m")
+    xr = [x.clone().requires_grad_(True) for x in xs]
+    y_r = torch.cat([O.patch_merging(x, sd, "m").reshape(-1, 4 * C) for x in xr])
     gy = torch.randn_like(y_r).to(BF16).float()
     (y_r * gy).sum().backward()
+    dx_r = torch.cat([x.grad.reshape(-1, C) for x in xr])
+    grp, r0 = [], 0
+    for B, S in sizes:
+        grp.append((B, S, S, r0))
+        r0 += B * S * S
     d = _dev()
-    xc, gc, bc = x.to(d).requires_grad_(True), g.to(d).requires_grad_(True), b.to(d).requires_grad_(True)
-    y = ops.PatchMergeLNFn.apply(xc, gc, bc, 1e-6, H, H)
+    xc = torch.cat([x.reshape(-1, C) for x in xs]).to(d).requires_grad_(True)
+    gc, bc = g.to(d).requires_grad_(True), b.to(d).requires_grad_(True)
+    y = ops.PatchMergeLNGroupsFn.apply(xc, gc, bc, 1e-6, tuple(grp))
     y.backward(gy.to(d).to(BF16))
     assert_close(y, y_r, 5e-3, "y")
-    assert_close(xc.grad, xr.grad, 1e-4, "dx")
+    assert_close(xc.grad, dx_r, 1e-4, "dx")
     assert_close(gc.grad, sd["m.norm.weight"].grad, 1e-4, "dgamma")
     assert_close(bc.grad, sd["m.norm.bias"].grad, 1e-4, "dbeta")
 
 
 @pytest.mark.parametrize("E,S", [(32, 48), (96, 96), (96, 224), (128, 112), (64, 40)])
-def test_patch_embed(E, S):
+def test_patch_embed_groups(E, S):
+    """two resolution groups written back to back (B = 2 images of S x S, then 1 of (S-8) x (S-8)): the second group's
+    row offset, and the weight / bias / LN gradients accumulated over both"""
     from esvit_b200 import ops
     from oracle import swin as O
     torch.manual_seed(E + S)
-    B = 2
-    img = torch.randn(B, 3, S, S)
+    imgs = [torch.randn(2, 3, S, S), torch.randn(1, 3, S - 8, S - 8)]
     sd = {"p.proj.weight": (torch.randn(E, 3, 4, 4) * 0.1), "p.proj.bias": torch.randn(E) * 0.1,
           "p.norm.weight": 1 + 0.1 * torch.randn(E), "p.norm.bias": 0.1 * torch.randn(E)}
     sdr = {k: v.clone().requires_grad_(True) for k, v in sd.items()}
-    y_r = O.patch_embed(img, sdr, "p", 4)
+    y_r = torch.cat([O.patch_embed(img, sdr, "p", 4).reshape(-1, E) for img in imgs])
     gy = torch.randn_like(y_r)
     (y_r * gy).sum().backward()
     d = _dev()
     ps = {k: v.to(d).requires_grad_(True) for k, v in sd.items()}
-    y = ops.PatchEmbedFn.apply(img.to(d), ps["p.proj.weight"], ps["p.proj.bias"], ps["p.norm.weight"],
-                               ps["p.norm.bias"], 1e-6)
+    y = ops.PatchEmbedGroupsFn.apply(ps["p.proj.weight"], ps["p.proj.bias"], ps["p.norm.weight"], ps["p.norm.bias"],
+                                     1e-6, *[img.to(d) for img in imgs])
     y.backward(gy.to(d))
     assert_close(y, y_r, TOL_FP32_KERNEL, "y")
     for k in sd:
@@ -165,17 +174,19 @@ def test_bias_gelu(R, N):
     assert_close(bc_.grad, br_.grad, 2e-3, "dbias")
 
 
-def test_token_mean():
+def test_token_mean_groups():
+    """two resolution groups back to back: 5 maps of 7 x 7, then 3 maps of 3 x 3"""
     from esvit_b200 import ops
     torch.manual_seed(0)
-    x = torch.randn(5, 49, 128)
+    xs = [torch.randn(5, 49, 128), torch.randn(3, 9, 128)]
     d = _dev()
-    xc = x.to(d).requires_grad_(True)
-    p = ops.TokenMeanFn.apply(xc)
-    g = torch.randn(5, 128)
+    xc = torch.cat([x.reshape(-1, 128) for x in xs]).to(d).requires_grad_(True)
+    p = ops.TokenMeanGroupsFn.apply(xc, ((5, 7, 7, 0), (3, 3, 3, 5 * 49)))
+    g = torch.randn(8, 128)
     p.backward(g.to(d))
-    assert_close(p, x.mean(1), 1e-6)
-    assert_close(xc.grad, (g / 49).unsqueeze(1).expand(5, 49, 128), 1e-6)
+    assert_close(p, torch.cat([x.mean(1) for x in xs]), 1e-6)
+    assert_close(xc.grad, torch.cat([(g[:5] / 49).repeat_interleave(49, 0), (g[5:] / 9).repeat_interleave(9, 0)]),
+                 1e-6)
 
 
 def test_gelu_l2norm_weightnorm():

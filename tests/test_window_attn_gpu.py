@@ -509,9 +509,9 @@ def test_reruns_are_bit_identical(name):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("ws,shift,C", [(7, 3, 96), (14, 7, 128)])
-def test_resolution_groups_equal_per_group_calls(ws, shift, C):
+def test_resolution_groups_equal_one_group_calls(ws, shift, C):
     """WindowAttentionGroupsFn over the step's layout (2 global 56² maps then 8 local 24² maps in one tensor, one shared
-    ws-7 expansion) against one WindowAttentionFn per group: out and dqkv bit-identical, the table / qkv-bias
+    ws-7 expansion) against one call per group on its own slice: out and dqkv bit-identical, the table / qkv-bias
     gradients (float atomics, accumulated over both groups) within fp32 summation noise"""
     from esvit_b200 import ops
     nH = C // HD
@@ -535,9 +535,8 @@ def test_resolution_groups_equal_per_group_calls(ws, shift, C):
     bexp = ops.expand_rel_pos_bias(table2, nH, ws)
     outs = []
     for B, H, W, r0 in groups:
-        o = ops.WindowAttentionFn.apply(qkv2[r0:r0 + B * H * W].view(B, H * W, 3 * C), bias2, table2, H, W, nH, ws,
-                                        shift, scale, bexp)
-        outs.append(o.reshape(-1, C))
+        outs.append(ops.WindowAttentionGroupsFn.apply(qkv2[r0:r0 + B * H * W], bias2, table2, ((B, H, W, 0),), nH, ws,
+                                                      shift, scale, bexp))
     out2 = torch.cat(outs)
     out2.backward(dout)
     assert torch.equal(out, out2)
