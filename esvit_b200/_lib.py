@@ -72,6 +72,14 @@ SIGNATURES = {
     "esvit_vil_sc_ws_floats": [I, I, I, I],
     "esvit_vil_sc_fwd": [P, P, P, P, P, P, P, P, I, I, I, I, F, P],
     "esvit_vil_sc_bwd": [P, P, P, P, P, P, P, P, P, P, P, P, P, P, P, I, I, I, I, F, P],
+    "esvit_vil_dense_parts": [I],
+    "esvit_vil_dense_fwd": [P, P, P, P, I, I, I, I, F, P],
+    "esvit_vil_dense_bwd": [P, P, P, P, P, P, P, P, P, I, I, I, I, F, P],
+    "esvit_vil_im2col": [P, P, I, I, I, I, I, I, I, I, P],
+    "esvit_vil_col2im": [P, P, I, I, I, I, I, I, I, I, P],
+    "esvit_vil_cls_cat_fwd": [P, P, P, I, I, I, P],
+    "esvit_vil_cls_cat_bwd": [P, P, P, I, I, I, I, P],
+    "esvit_vil_bias_spmv": [P, P, P, P, P, P, I, I, P, I, P],
     "esvit_vit_patches": [P, P, I, I, I, P],
     "esvit_vit_tokens_fwd": [P, P, P, P, I, I, I, P],
     "esvit_vit_tokens_bwd": [P, P, P, P, P, I, I, I, I, P],
@@ -174,6 +182,8 @@ _META = {
                                      "nH": int(a[11])},
     "esvit_vil_sc_fwd": lambda a: {"B": int(a[8]), "nx": int(a[9]), "ny": int(a[10]), "nH": int(a[11])},
     "esvit_vil_sc_bwd": lambda a: {"B": int(a[15]), "nx": int(a[16]), "ny": int(a[17]), "nH": int(a[18])},
+    "esvit_vil_dense_fwd": lambda a: {"B": int(a[4]), "L": int(a[5]), "C": int(a[6]), "nH": int(a[7])},
+    "esvit_vil_dense_bwd": lambda a: {"B": int(a[9]), "L": int(a[10]), "C": int(a[11]), "nH": int(a[12])},
     "esvit_mhsa_fwd": lambda a: {"B": int(a[3]), "L": int(a[4]), "C": int(a[5]), "nH": int(a[6])},
     "esvit_mhsa_bwd": lambda a: {"B": int(a[6]), "L": int(a[7]), "C": int(a[8]), "nH": int(a[9])},
     "esvit_vit_tokens_bwd": lambda a: {"B": int(a[-5]), "N": int(a[-4]), "D": int(a[-3])},

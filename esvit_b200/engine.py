@@ -21,6 +21,7 @@ from . import ops, utils
 from .losses import DDINOLoss, DINOLoss
 from .optim import FusedAdamWEMA
 from . import cvt_v4_transformer as cvts
+from . import vision_longformer as vils
 from . import vision_transformer as vits
 from .swin_transformer import SwinTransformer
 from .vision_transformer import DINOHead
@@ -45,18 +46,26 @@ CVT_SPECS = {
     "cvt_13": dict(cvt_spec=cvts.S1_SPEC, drop_path_rate=0.1),
 }
 
+# Vision Longformer (main_esvit.py:257-276 with the README's vil_2262 arch): `vil_spec` holds MsViT's arguments
+VIL_SPECS = {
+    "vil_2262": dict(vil_spec=vils.VIL_2262, drop_path_rate=0.1),
+}
+
 
 def build_network(spec: dict, out_dim: int, use_dense_prediction: bool, is_teacher: bool = False,
                   norm_last_layer: bool = True, img_size: int = 224, head_kwargs: Optional[dict] = None) -> nn.Module:
     """What main_esvit.py:235-254 (Swin) / :304-327 (ViT, a spec with `vit_arch`) / :280-301 (CvT, a spec with
-    `cvt_spec`) builds: the backbone (teacher:
+    `cvt_spec`) / :257-276 (ViL, a spec with `vil_spec`; num_features = out_planes) builds: the backbone (teacher:
     drop_path 0) + DINOHead(s) assigned to ``.head`` / ``.head_dense``."""
     spec = dict(spec)
     if is_teacher:
         spec["drop_path_rate"] = 0.0
     vit_arch = spec.pop("vit_arch", None)
     cvt_spec = spec.pop("cvt_spec", None)
-    if cvt_spec is not None:
+    vil_spec = spec.pop("vil_spec", None)
+    if vil_spec is not None:
+        net = vils.msvit(vil_spec, 0, use_dense_prediction, drop_path_rate=spec["drop_path_rate"])
+    elif cvt_spec is not None:
         net = cvts.cvt(cvt_spec, 0, use_dense_prediction, drop_path_rate=spec["drop_path_rate"])
     elif vit_arch is not None:
         net = vits.__dict__[vit_arch](img_size=[img_size], use_dense_prediction=use_dense_prediction, **spec)
@@ -253,7 +262,7 @@ def make_step(arch: str = "swin_tiny_w7", out_dim: int = 65536, ncrops: int = 10
     """Build student/teacher/loss/optimizer the way train_esvit does (main_esvit.py:235-435) and return
     (step, student, teacher, loss)."""
     if spec is None:
-        spec = VIT_SPECS.get(arch) or CVT_SPECS.get(arch) or SWIN_SPECS[arch]
+        spec = VIT_SPECS.get(arch) or CVT_SPECS.get(arch) or VIL_SPECS.get(arch) or SWIN_SPECS[arch]
     spec = dict(spec)
     if drop_path is not None:
         spec["drop_path_rate"] = drop_path

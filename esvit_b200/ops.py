@@ -1252,19 +1252,259 @@ class SlidingChunkAttnFn(Function):
         q, kv, bias, bias_g, mode, out, lse, lse_g = ctx.saved_tensors
         B, nx, ny, nH, scale = ctx.meta
         g = _chk(g, BF16, "g").contiguous()
-        key = (q.device, B, nx, ny, nH)
-        ws = _vil_ws.get(key)
-        if ws is None:
-            n = _lib.load().esvit_vil_sc_ws_floats(B, nx, ny, nH)
-            if n <= 0:
-                raise ValueError("esvit_vil_sc_bwd: problem too large for the workspace")
-            ws = _vil_ws[key] = torch.empty(n, dtype=F32, device=q.device)
+        ws = _vil_sc_ws(q.device, B, nx, ny, nH)
         dq, dkv = torch.empty_like(q), torch.empty_like(kv)
         dvec = torch.empty_like(lse)
         dbias, dbias_g = torch.empty_like(bias), torch.empty_like(bias_g)
         _lib.call("esvit_vil_sc_bwd", _p(q), _p(kv), _p(bias), _p(bias_g), _p(mode), _p(out), _p(g), _p(lse), _p(lse_g),
                   _p(dvec), _p(ws), _p(dq), _p(dkv), _p(dbias), _p(dbias_g), B, nx, ny, nH, scale, _stream())
         return dq, dkv, dbias, dbias_g, None, None, None, None, None, None
+
+
+def _vil_sc_ws(device, B: int, nx: int, ny: int, nH: int) -> Tensor:
+    key = (device, B, nx, ny, nH)
+    ws = _vil_ws.get(key)
+    if ws is None:
+        n = _lib.load().esvit_vil_sc_ws_floats(B, nx, ny, nH)
+        if n <= 0:
+            raise ValueError("esvit_vil_sc_bwd: problem too large for the workspace")
+        ws = _vil_ws[key] = torch.empty(n, dtype=F32, device=device)
+    return ws
+
+
+class SlidingChunkAttnGroupsFn(Function):
+    """SlidingChunkAttnFn over resolution groups stored back to back: q bf16 [T, C], kv bf16 [T, 2C] (the query / kv
+    GEMM outputs incl. bias over every row of every image), group g = (B, nx, ny, row0, bias_off, bias_g_off) = rows
+    [row0, row0 + B*(1 + nx*ny)).  bias: ONE fp32 vector (RelBiasFn's output) holding every group's [nH, 49, 442] local
+    bias at bias_off and its [nH, N] global-row bias at bias_g_off; modes int32 [G] on the device, element g the mode
+    of group g.  One esvit_vil_sc_fwd / _bwd per group on pointer offsets.  The bias gradient of group g is written into
+    the same offsets of one gradient vector (the kernel writes, it does not accumulate; RelBiasFn's backward sums the
+    groups in a fixed order).  q_bias / kv_bias (fp32 or None) only receive their gradients: column sums of dq / dkv."""
+
+    @staticmethod
+    def forward(ctx, q, kv, q_bias, kv_bias, bias, modes, groups, num_heads: int, scale: float):
+        q, kv = _chk(q, BF16, "q"), _chk(kv, BF16, "kv")
+        bias = _chk(bias, F32, "bias")
+        modes = _chk(modes, torch.int32, "modes")
+        T, C = q.shape
+        if C != 32 * num_heads or kv.shape != (T, 2 * C):
+            raise ValueError(f"q [T, 32 nH] and kv [T, 2C] required, got {tuple(q.shape)}, {tuple(kv.shape)}")
+        if sum(B * (1 + nx * ny) for B, nx, ny, _, _, _ in groups) != T or modes.numel() != len(groups):
+            raise ValueError(f"groups {groups} do not cover the {T} rows, or not one mode per group")
+        out = torch.empty(T, C, dtype=BF16, device=q.device)
+        lse_off, lse_g_off, n, ng = [], [], 0, 0
+        for B, nx, ny, _, _, _ in groups:
+            lse_off.append(n)
+            lse_g_off.append(ng)
+            n += B * num_heads * (-(-nx // VIL_W)) * (-(-ny // VIL_W)) * VIL_W * VIL_W
+            ng += B * num_heads
+        lse = torch.empty(n, dtype=F32, device=q.device)
+        lse_g = torch.empty(ng, dtype=F32, device=q.device)
+        for gi, ((B, nx, ny, r0, bo, bgo), lo, lgo) in enumerate(zip(groups, lse_off, lse_g_off)):
+            _lib.call("esvit_vil_sc_fwd", _po(q, r0 * C), _po(kv, r0 * 2 * C), _po(bias, bo), _po(bias, bgo),
+                      _po(modes, gi), _po(out, r0 * C), _po(lse, lo), _po(lse_g, lgo), B, nx, ny, num_heads, scale,
+                      _stream())
+        ctx.save_for_backward(q, kv, bias, modes, out, lse, lse_g)
+        ctx.meta = (tuple(groups), tuple(lse_off), tuple(lse_g_off), num_heads, scale, q_bias is not None,
+                    kv_bias is not None)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        q, kv, bias, modes, out, lse, lse_g = ctx.saved_tensors
+        groups, lse_off, lse_g_off, nH, scale, has_qb, has_kvb = ctx.meta
+        g = _chk(g, BF16, "g")
+        C = q.shape[1]
+        dq, dkv = torch.empty_like(q), torch.empty_like(kv)
+        dvec = torch.empty_like(lse)
+        dbias = torch.zeros_like(bias)  # every group writes its own slots; the zeros cover nothing but alignment gaps
+        for gi, ((B, nx, ny, r0, bo, bgo), lo, lgo) in enumerate(zip(groups, lse_off, lse_g_off)):
+            ws = _vil_sc_ws(q.device, B, nx, ny, nH)
+            _lib.call("esvit_vil_sc_bwd", _po(q, r0 * C), _po(kv, r0 * 2 * C), _po(bias, bo), _po(bias, bgo),
+                      _po(modes, gi), _po(out, r0 * C), _po(g, r0 * C), _po(lse, lo), _po(lse_g, lgo), _po(dvec, lo),
+                      _p(ws), _po(dq, r0 * C), _po(dkv, r0 * 2 * C), _po(dbias, bo), _po(dbias, bgo), B, nx, ny, nH,
+                      scale, _stream())
+        return (dq, dkv, colsum(dq) if has_qb else None, colsum(dkv) if has_kvb else None, dbias,
+                None, None, None, None)
+
+
+class DenseBiasAttnGroupsFn(Function):
+    """Whole-sequence attention at head dim 32 with an additive bias (vision_longformer.py Attention.forward :86-131)
+    over resolution groups stored back to back: qkv bf16 [T, 3C] (qkv GEMM output incl. bias), group g = (B, L, row0,
+    bias_off) = rows [row0, row0 + B*L), bias fp32 [nH, L, L] at bias_off of ONE vector (RelBiasFn's output).  One
+    esvit_vil_dense_fwd / _bwd per group; each group's bias gradient (sum over its images, fixed order) is written at the
+    same offset of one gradient vector.  qkv_bias only receives its gradient: the column sums of dqkv."""
+
+    @staticmethod
+    def forward(ctx, qkv, qkv_bias, bias, groups, num_heads: int, scale: float):
+        qkv, bias = _chk(qkv, BF16, "qkv"), _chk(bias, F32, "bias")
+        T, C3 = qkv.shape
+        C = C3 // 3
+        if sum(B * L for B, L, _, _ in groups) != T:
+            raise ValueError(f"groups {groups} do not cover the {T} rows of qkv")
+        out = torch.empty(T, C, dtype=BF16, device=qkv.device)
+        lse = torch.empty(T * num_heads, dtype=F32, device=qkv.device)  # per group [B, nH, L] at row0 * nH
+        for B, L, r0, bo in groups:
+            _lib.call("esvit_vil_dense_fwd", _po(qkv, r0 * C3), _po(bias, bo), _po(out, r0 * C), _po(lse, r0 * num_heads),
+                      B, L, C, num_heads, scale, _stream())
+        ctx.save_for_backward(qkv, bias, out, lse)
+        ctx.meta = (tuple(groups), num_heads, scale, qkv_bias is not None)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        qkv, bias, out, lse = ctx.saved_tensors
+        groups, nH, scale, has_bias = ctx.meta
+        g = _chk(g, BF16, "g")
+        C = qkv.shape[1] // 3
+        dqkv = torch.empty_like(qkv)
+        dvec = torch.empty_like(lse)
+        dbias = torch.zeros_like(bias)
+        lib = _lib.load()
+        for B, L, r0, bo in groups:
+            part = torch.empty(lib.esvit_vil_dense_parts(B) * nH * L * L, dtype=F32, device=qkv.device)
+            _lib.call("esvit_vil_dense_bwd", _po(qkv, r0 * 3 * C), _po(bias, bo), _po(out, r0 * C), _po(g, r0 * C),
+                      _po(lse, r0 * nH), _po(dvec, r0 * nH), _p(part), _po(dqkv, r0 * 3 * C), _po(dbias, bo), B, L, C, nH,
+                      scale, _stream())
+        return dqkv, (colsum(dqkv) if has_bias else None), dbias, None, None, None
+
+
+def vil_dense_attention(qkv: Tensor, bias: Tensor, num_heads: int, scale: float) -> Tuple[Tensor, Tensor]:
+    """(out bf16 [B*L, C], lse fp32 [B, nH, L]) of DenseBiasAttnGroupsFn's kernel on qkv bf16 [B, L, 3C] and bias fp32
+    [nH, L, L]; not differentiable."""
+    qkv, bias = _chk(qkv, BF16, "qkv"), _chk(bias, F32, "bias")
+    B, L, C3 = qkv.shape
+    out = torch.empty(B * L, C3 // 3, dtype=BF16, device=qkv.device)
+    lse = torch.empty(B, num_heads, L, dtype=F32, device=qkv.device)
+    _lib.call("esvit_vil_dense_fwd", _p(qkv), _p(bias), _p(out), _p(lse), B, L, C3 // 3, num_heads, scale, _stream())
+    return out, lse
+
+
+class VilStreamEmbedFn(Function):
+    """PatchEmbed.proj (Conv2d p x p / p, vision_longformer.py:203-204) of stages 2-4, reading the previous stage's
+    residual stream x fp32 [T, Cin] directly: group g = (B, N, off, H, W, row0) holds B images of N rows each at rows
+    [row0, row0 + B*N), the H x W map rows of an image start at row `off` (the global rows before it are dropped,
+    forward_features :584-592).  All groups -> one im2col buffer bf16 [sum B*(H/p)*(W/p), Kp] -> ONE GEMM with the bias
+    -> bf16 [rows, Cout].  bias gets its gradient from the consumer (the fused add + LN).  backward: the fp32 weight
+    gradient and dx (0 on the global rows)."""
+
+    @staticmethod
+    def forward(ctx, x, weight, w16, bias, groups, p: int):
+        x, w16 = _chk(x, F32, "x"), _chk(w16, BF16, "w16")
+        Cout, Kp = w16.shape
+        Cin = x.shape[1]
+        if tuple(weight.shape) != (Cout, Cin, p, p):
+            raise ValueError(f"weight {tuple(weight.shape)} is not [{Cout}, {Cin}, {p}, {p}]")
+        n = [B * (H // p) * (W // p) for B, N, off, H, W, r0 in groups]
+        # the im2col writes the K = Cin*p*p columns; padding columns (Kp > K) must be zeros, not garbage
+        alloc = torch.empty if Kp == Cin * p * p else torch.zeros
+        rows = alloc(sum(n), Kp, dtype=BF16, device=x.device)
+        o0 = 0
+        for (B, N, off, H, W, r0), ni in zip(groups, n):
+            _lib.call("esvit_vil_im2col", _po(x, r0 * Cin), _po(rows, o0 * Kp), B, N, off, Cin, H, W, p, Kp, _stream())
+            o0 += ni
+        y = gemm(rows, w16, bias)
+        ctx.save_for_backward(rows, w16)
+        ctx.meta = (tuple(weight.shape), tuple(x.shape), tuple(groups), tuple(n), p)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        rows, w16 = ctx.saved_tensors
+        wshape, xshape, groups, n, p = ctx.meta
+        g = _chk(g, BF16, "g")
+        K = wshape[1] * p * p
+        dw = None
+        if ctx.needs_input_grad[1]:
+            dw = gemm_wgrad(g, rows)
+            dw = (dw[:, :K].contiguous() if dw.shape[1] != K else dw).view(wshape)
+        dx = None
+        if ctx.needs_input_grad[0]:
+            drows = gemm(g, w16, None, b_mn=True)
+            Kp, Cin = drows.shape[1], xshape[1]
+            dx = torch.empty(xshape, dtype=F32, device=g.device)
+            o0 = 0
+            for (B, N, off, H, W, r0), ni in zip(groups, n):
+                _lib.call("esvit_vil_col2im", _po(drows, o0 * Kp), _po(dx, r0 * Cin), B, N, off, Cin, H, W, p, Kp,
+                          _stream())
+                o0 += ni
+        return dx, dw, None, None, None, None
+
+
+class ClsCatGroupsFn(Function):
+    """PatchEmbed's cat(cls_token, x) (vision_longformer.py:240-243) over resolution groups: y fp32 [sum B*n, C] (the
+    embedding LN output, groups back to back) -> the residual stream fp32 [sum B*(1+n), C]; groups = ((B, n), ...).
+    The cls_token gradient is the fixed-order sum of the global rows' gradient."""
+
+    @staticmethod
+    def forward(ctx, y, cls_token, groups):
+        y, cls = _chk(y, F32, "y"), _chk(cls_token, F32, "cls_token")
+        C = y.shape[1]
+        out = torch.empty(sum(B * (1 + n) for B, n in groups), C, dtype=F32, device=y.device)
+        y0 = x0 = 0
+        for B, n in groups:
+            _lib.call("esvit_vil_cls_cat_fwd", _po(y, y0 * C), _p(cls), _po(out, x0 * C), B, n, C, _stream())
+            y0 += B * n
+            x0 += B * (1 + n)
+        ctx.meta = (tuple(groups), tuple(y.shape), tuple(cls_token.shape))
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        groups, yshape, cshape = ctx.meta
+        g = _chk(g, F32, "g")
+        C = yshape[1]
+        dy = torch.empty(yshape, dtype=F32, device=g.device)
+        dcls = torch.empty(cshape, dtype=F32, device=g.device)
+        y0 = x0 = 0
+        for gi, (B, n) in enumerate(groups):
+            _lib.call("esvit_vil_cls_cat_bwd", _po(g, x0 * C), _po(dy, y0 * C), _p(dcls), B, n, C, 1 if gi else 0,
+                      _stream())
+            y0 += B * n
+            x0 += B * (1 + n)
+        return dy, dcls, None
+
+
+class RelBiasFn(Function):
+    """The relative-position biases of one ViL attention module for every resolution group, as ONE fp32 vector
+    y = M . [table | g2l | g2g] (flattened parameters): M is a sparse matrix built once per geometry on the host
+    (vision_longformer.bias_plan: gathers, and at other resolutions than the table's the reference's bicubic resize as
+    fixed per-axis weights).  backward: d[table | g2l | g2g] = M^T . dy, a gather-sum in a fixed order per parameter
+    entry (the transposed CSR), so no atomics.  plan = (M CSR (rowptr, col, val), M^T CSR, nrows) on the device."""
+
+    @staticmethod
+    def forward(ctx, table, g2l, g2g, plan):
+        table = _chk(table, F32, "table")
+        g2l, g2g = _chk(g2l, F32, "g2l"), _chk(g2g, F32, "g2g")
+        (rp, col, val), _, nrows = plan
+        n0, n1 = table.numel(), (g2l.numel() if g2l is not None else 0)
+        y = torch.empty(nrows, dtype=F32, device=table.device)
+        _lib.call("esvit_vil_bias_spmv", _p(rp), _p(col), _p(val), _p(table), _p(g2l), _p(g2g), n0, n1, _p(y), nrows,
+                  _stream())
+        ctx.plan = plan
+        ctx.shapes = (tuple(table.shape), None if g2l is None else tuple(g2l.shape),
+                      None if g2g is None else tuple(g2g.shape))
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        g = _chk(g, F32, "g")
+        _, (rp, col, val), _ = ctx.plan
+        shapes = ctx.shapes
+        sizes = [0 if s is None else int(torch.Size(s).numel()) for s in shapes]
+        d = torch.empty(sum(sizes), dtype=F32, device=g.device)
+        _lib.call("esvit_vil_bias_spmv", _p(rp), _p(col), _p(val), _p(g), None, None, g.numel(), 0, _p(d), d.numel(),
+                  _stream())
+        out, o = [], 0
+        for s, n in zip(shapes, sizes):
+            out.append(None if s is None else d[o:o + n].view(s))
+            o += n
+        return out[0], out[1], out[2], None
 
 
 # ------------------------------------------------------------------------------------------------------------

@@ -261,6 +261,34 @@ int esvit_vil_sc_bwd(const void* q, const void* kv, const float* bias, const flo
                      void* dq, void* dkv, float* dbias, float* dbias_g, int B, int nx, int ny, int nH, float scale,
                      void* stream);
 
+/* ---- Vision Longformer dense stages, embedding and bias assembly (vil_dense.cu) ------------------------------------
+ * vil_dense_fwd / _bwd: multi-head attention at head dim 32 with an additive fp32 bias [nH, L, L] (vision_longformer.py
+ *   Attention.forward :86-131), L <= 256.  qkv / dqkv bf16 [B*L, 3C] ([q|k|v][head][32]), out / dout bf16 [B*L, C],
+ *   lse / dvec fp32 [B, nH, L], part fp32 scratch [esvit_vil_dense_parts(B), nH, L, L]; dbias fp32 [nH, L, L] is written
+ *   (sum over the images of dS, fixed order).  No floating-point atomics.
+ * vil_im2col: rows bf16 [B*(H/p)*(W/p), Kp] of the p x p / p conv over per-image token rows x fp32 [B*N, Cin] whose
+ *   H*W map rows start at row off of each image (the global rows skipped); column c*p*p + ky*p + kx.  col2im: dx fp32
+ *   [B*N, Cin] fully written (0 on the global rows).
+ * vil_cls_cat_fwd: out fp32 [B*(1+n), C] = per image cat(cls [C], y rows [n, C]).  _bwd: dy = the patch rows of g;
+ *   dcls (+)= sum over the images of the global rows of g (accumulate != 0 adds to dcls).  C % 4 == 0.
+ * vil_bias_spmv: y[r] = sum_k val[k] * src(col[k]) over k in [rowptr[r], rowptr[r+1]) in order (CSR, int32), with
+ *   src(c) = s0[c] for c < n0, s1[c - n0] for c < n0 + n1, else s2[c - n0 - n1].  The relative-position bias gathers and
+ *   bicubic resizes, and their transposes (fixed-order gather-sums), are such maps. */
+int esvit_vil_dense_parts(int B);
+int esvit_vil_dense_fwd(const void* qkv, const float* bias, void* out, float* lse, int B, int L, int C, int nH,
+                        float scale, void* stream);
+int esvit_vil_dense_bwd(const void* qkv, const float* bias, const void* out, const void* dout, const float* lse,
+                        float* dvec, float* part, void* dqkv, float* dbias, int B, int L, int C, int nH, float scale,
+                        void* stream);
+int esvit_vil_im2col(const float* x, void* rows, int B, int N, int off, int Cin, int H, int W, int p, int Kp,
+                     void* stream);
+int esvit_vil_col2im(const void* drows, float* dx, int B, int N, int off, int Cin, int H, int W, int p, int Kp,
+                     void* stream);
+int esvit_vil_cls_cat_fwd(const float* y, const float* cls, float* out, int B, int n, int C, void* stream);
+int esvit_vil_cls_cat_bwd(const float* g, float* dy, float* dcls, int B, int n, int C, int accumulate, void* stream);
+int esvit_vil_bias_spmv(const int* rowptr, const int* col, const float* val, const float* s0, const float* s1,
+                        const float* s2, int n0, int n1, float* y, int nrows, void* stream);
+
 /* ---- optimiser-side multi-tensor kernels (host arrays of device pointers) ----------------------------------
  * ema_multi: teacher = teacher*m + student*(1-m), bit-exact with main_esvit.py:587-590.
  * clip_multi: per-tensor L2 clip of utils.py:106-115; sumsq_ws double[n] workspace; norms fp32[n] or NULL. */
