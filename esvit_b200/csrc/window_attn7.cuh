@@ -7,16 +7,14 @@
 //
 // Instruction diet (the first version issued ~40 instructions per score element):
 //   * scores live in the log2 domain: s' = acc*(scale*log2e) + bias*log2e (one FMA), P = ex2(s' - m');
-//   * the rel-pos bias of this head is expanded ONCE per persistent CTA - forward: straight into the accumulator
-//     fragment layout in registers; backward: into a [64][72] fp32 shared-memory table - with -inf in the padded
-//     rows/columns, which also replaces every bounds check;
+//   * the rel-pos bias of this head is loaded ONCE per persistent CTA, straight into the accumulator fragment layout in
+//     registers (forward and backward), with -inf in the padded rows/columns, which also replaces every bounds check;
 //   * the shift mask is a template flag, so un-shifted blocks carry no mask code.
 #pragma once
 #include "wa_common.cuh"
 
 namespace wa {
 
-constexpr int BLD = 72;        // row stride (floats) of the expanded bias table: 72 % 32 == 8 -> conflict-free float2 reads
 constexpr int TILE7 = 64 * LD;  // bf16 elements of one 64-row tile
 
 // Rel-pos bias of every head expanded ONCE per call to a dense [nH][64][64] fp32 table in the log2 domain with -inf in
@@ -233,12 +231,26 @@ __global__ void __launch_bounds__(128, 4) window_attn_fwd7_kernel(
 static size_t fwd7_smem() { return (size_t)2 * 3 * TILE7 * 2 + (size_t)4 * 64 * 4; }
 
 // ------------------------------------------------------------------------------------------------
-// backward: no shared-memory transposition and no atomics in the inner loop.
-//   phase A  warp = 16-query tile : S, P, dP, dS  -> dQ = dS K ;  dS also summed into register accumulators
+// backward: one pass over P and dS, no atomics in the window loop, dqkv written as whole 64-byte head rows.
+//   phase A  warp = 16-query tile : D = rowsum(dO * O) of its rows, S, P, dP, dS; bf16 P and dS go to shared memory
+//                                   -> dQ = dS K; dS is also summed into register accumulators
 //                                   (this warp's queries x all keys, over all windows) = rel-pos-bias gradient
-//   phase B  warp = 16-key tile   : S^T = K Q^T, P^T, dP^T = V dO^T, dS^T recomputed in the transposed layout
-//                                   -> dV = P^T dO, dK = dS^T Q straight from the accumulator fragments
-// qkv-bias gradients are the column sums of dQ / dK / dV over all 49 slots (padded ones included).
+//   phase B  warp = 16-key tile   : P^T and dS^T come back through ldmatrix.trans -> dV = P^T dO, dK = dS^T Q
+//   store                         : dQ / dK / dV tiles are staged as bf16 in the O / K / V tiles of the stage (dead by then)
+//                                   and leave as 16-byte vectors, four lanes per head row, real tokens only
+// qkv-bias gradients are the column sums of dQ / dK / dV over all 49 slots (padded ones included), accumulated per
+// thread over the window loop and reduced once per CTA.
+constexpr int PLD = 72;  // row stride (bf16) of the P / dS tiles: 144 B rows -> conflict-free fragment stores and ldmatrix.trans
+
+// column sums of a 16 x 32 fp32 accumulator tile (4 d-tiles x C-fragment), this thread's two rows, added to acc[8]
+__device__ __forceinline__ void colsum_acc(const float (&t)[4][4], float (&acc)[8]) {
+#pragma unroll
+  for (int dt = 0; dt < 4; dt++) {
+    acc[2 * dt] += t[dt][0] + t[dt][2];
+    acc[2 * dt + 1] += t[dt][1] + t[dt][3];
+  }
+}
+
 template <bool SHIFT>
 __global__ void __launch_bounds__(128, 3) window_attn_bwd7_kernel(
     const bf16* __restrict__ qkv, const bf16* __restrict__ qkv_bias, const float* __restrict__ bexp,
@@ -251,79 +263,91 @@ __global__ void __launch_bounds__(128, 3) window_attn_bwd7_kernel(
   // 2 CTAs/SM at the 128-register cap lose more than the halved per-window latency gains)
   constexpr int NTHREADS = 128;
   static_assert(C::KP == 64 && C::NW == 4, "fast path assumes a 64-slot window and 4 tiles per phase");
+  static_assert((C::NB + 3) % 4 == 0, "the 16-byte bias chunks follow the float arrays");
   extern __shared__ __align__(16) unsigned char smraw[];
   bf16* tiles = reinterpret_cast<bf16*>(smraw);                       // [2 stages][Q | K | V | dO | O]
-  float* bm = reinterpret_cast<float*>(tiles + 2 * 5 * TILE7);         // [64][BLD] expanded bias (log2 domain, -inf pad)
-  float* dbt = bm + C::KP * BLD;                                      // [NB] bias-gradient bins
-  float* dqb = dbt + C::NB + 1;                                       // [3][32] (+1: NB is odd, keep 8-byte alignment)
-  float* Dsm = dqb + 3 * HD;                                          // [64] rowsum(dO * O)
-  float* Lrawb = Dsm + C::KP;                                         // [2][64] natural-log lse of the stage
+  bf16* Ps = tiles + 2 * 5 * TILE7;                                   // [64][PLD] P  (rows = queries)
+  bf16* dSs = Ps + C::KP * PLD;                                       // [64][PLD] dS (rows = queries)
+  float* dbt = reinterpret_cast<float*>(dSs + C::KP * PLD);           // [NB] bias-gradient bins
+  float* dqb = dbt + C::NB + 3;                                       // [3][32] (+3: keeps everything below 16-byte aligned)
+  float* Lrawb = dqb + 3 * HD;                                        // [2][64] natural-log lse of the stage
   int* tokb = reinterpret_cast<int*>(Lrawb + 2 * 64);                 // [2][64]
   int* ridb = tokb + 2 * 64;                                          // [2][64]
+  uint4* bsm = reinterpret_cast<uint4*>(ridb + 2 * 64);               // [3][4] qkv bias of head h as 16-byte chunks
+  float* vsum = reinterpret_cast<float*>(bsm + 3 * 4) + threadIdx.x;  // [8][NTHREADS] this thread's column sums of dV
 
   const int h = blockIdx.x;  // heads fastest: the nH CTAs sharing a window's token rows run together (DRAM page locality)
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   int win = blockIdx.y, stage = 0;
-  uint4 bchunk[3];
+  {
+    // the forward keeps a thread's three bias chunks in registers over the window loop; here they are re-read from
+    // shared memory at every gather, which leaves those 12 registers to the accumulators
+    uint4 bchunk[3];
 #pragma unroll
-  for (int part = 0; part < 3; part++)
-    bchunk[part] = __ldg(reinterpret_cast<const uint4*>(qkv_bias + part * g.C + h * HD + (threadIdx.x & 3) * 8));
-  if (win < nwin_total) issue7<true, NTHREADS>(g, win, h, qkv, bchunk, dout, out, lse, tiles, Lrawb, tokb, ridb);
-  cp_async_commit();
+    for (int part = 0; part < 3; part++) {
+      bchunk[part] = __ldg(reinterpret_cast<const uint4*>(qkv_bias + part * g.C + h * HD + (threadIdx.x & 3) * 8));
+      if (threadIdx.x < 4) bsm[part * 4 + threadIdx.x] = bchunk[part];
+    }
+    if (win < nwin_total) issue7<true, NTHREADS>(g, win, h, qkv, bchunk, dout, out, lse, tiles, Lrawb, tokb, ridb);
+    cp_async_commit();
+  }
 
-  for (int i = threadIdx.x; i < C::KP * C::KP / 4; i += NTHREADS) {  // copy the expanded table of head h (float4)
-    const int row = i >> 4, c4 = (i & 15) * 4;
-    float4 v = __ldg(reinterpret_cast<const float4*>(bexp + (long long)h * 4096 + row * 64 + c4));
-    if (row >= C::NT) v = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);  // padded query rows: P = 0
-    *reinterpret_cast<float4*>(bm + row * BLD + c4) = v;
+  const int r0 = warp * 16;                       // this warp's query tile (phase A) / key tile (phase B)
+  const int rA = r0 + (lane >> 2), rB = rA + 8;
+  const int frag_off = (r0 + (lane & 7) + ((lane >> 3) & 1) * 8) * LD + (lane >> 4) * 8;  // A-fragment rows of the tile
+  // rel-pos bias of (head h, this warp's 16 query rows) in accumulator-fragment layout, as in the forward; padded
+  // query rows are -inf throughout (P = 0)
+  float breg[C::NT8][4];
+  {
+    const float* bh = bexp + (long long)h * 4096 + (lane & 3) * 2;
+#pragma unroll
+    for (int nt = 0; nt < C::NT8; nt++) {
+      float2 a = __ldg(reinterpret_cast<const float2*>(bh + rA * 64 + nt * 8));
+      float2 b = __ldg(reinterpret_cast<const float2*>(bh + rB * 64 + nt * 8));
+      if (rA >= C::NT) a = make_float2(-INFINITY, -INFINITY);
+      if (rB >= C::NT) b = make_float2(-INFINITY, -INFINITY);
+      breg[nt][0] = a.x; breg[nt][1] = a.y; breg[nt][2] = b.x; breg[nt][3] = b.y;
+    }
   }
   for (int i = threadIdx.x; i < C::NB; i += NTHREADS) dbt[i] = 0.f;
   for (int i = threadIdx.x; i < 3 * HD; i += NTHREADS) dqb[i] = 0.f;
   float dsacc[C::NT8][4];
 #pragma unroll
   for (int nt = 0; nt < C::NT8; nt++) dsacc[nt][0] = dsacc[nt][1] = dsacc[nt][2] = dsacc[nt][3] = 0.f;
+  // column sums of dQ / dK / dV (unscaled) over this thread's rows of every window: dQ / dK in registers, dV in shared
+  // memory (8 more accumulators do not fit the 168 registers of 3 CTAs per SM without spilling)
+  float csum[2][8];
+#pragma unroll
+  for (int i = 0; i < 8; i++) {
+    csum[0][i] = csum[1][i] = 0.f;
+    vsum[i * NTHREADS] = 0.f;
+  }
 
   const float c = scale * LOG2E;
-  const int r0 = warp * 16;                       // this warp's query tile (phase A) / key tile (phase B)
-  const int rA = r0 + (lane >> 2), rB = rA + 8;
-  const int frag_off = (r0 + (lane & 7) + ((lane >> 3) & 1) * 8) * LD + (lane >> 4) * 8;  // A-fragment rows of the tile
+  __syncthreads();  // bsm is read by every thread at the first gather of the loop
 
   for (; win < nwin_total; win += gridDim.y, stage ^= 1) {
     const int nxt = win + gridDim.y;
-    if (nxt < nwin_total)
+    if (nxt < nwin_total) {
+      uint4 bchunk[3];
+#pragma unroll
+      for (int part = 0; part < 3; part++) bchunk[part] = bsm[part * 4 + (threadIdx.x & 3)];
       issue7<true, NTHREADS>(g, nxt, h, qkv, bchunk, dout, out, lse, tiles + (stage ^ 1) * 5 * TILE7, Lrawb + (stage ^ 1) * 64,
                    tokb + (stage ^ 1) * 64, ridb + (stage ^ 1) * 64);
+    }
     cp_async_commit();
     cp_async_wait<1>();
     __syncthreads();
-    const bf16* Qs = tiles + stage * 5 * TILE7;
-    const bf16* Ks = Qs + TILE7;
-    const bf16* Vs = Ks + TILE7;
-    const bf16* dOs = Vs + TILE7;
-    const bf16* Os = dOs + TILE7;
+    bf16* Qs = tiles + stage * 5 * TILE7;
+    bf16* Ks = Qs + TILE7;   // dK staging after phase A
+    bf16* Vs = Ks + TILE7;   // dV staging after phase A
+    bf16* dOs = Vs + TILE7;
+    bf16* Os = dOs + TILE7;  // rows of a query tile: dQ staging once its warp has formed D
     const float* Lraw = Lrawb + stage * 64;
     const int* tok = tokb + stage * 64;
     const int* rid = ridb + stage * 64;
     if (g.dbg == 2) { __syncthreads(); continue; }
-    {  // D[t] = rowsum(dO * O): two threads per row
-      const int t = threadIdx.x >> 1, half = threadIdx.x & 1;
-      float part = 0.f;
-#pragma unroll
-      for (int k = 0; k < 2; k++) {
-        float fd[8], fo[8];
-        unpack8(*reinterpret_cast<const bf16x8*>(dOs + t * LD + half * 16 + k * 8), fd);
-        unpack8(*reinterpret_cast<const bf16x8*>(Os + t * LD + half * 16 + k * 8), fo);
-#pragma unroll
-        for (int j = 0; j < 8; j++) part += fd[j] * fo[j];
-      }
-      part += __shfl_xor_sync(0xffffffffu, part, 1);
-      if (half == 0) Dsm[t] = part;
-    }
-    __syncthreads();
 
-    const int tA = rA < C::NT ? tok[rA] : -1, tB = rB < C::NT ? tok[rB] : -1;
-    int ridA = 0, ridB = 0;
-    if (SHIFT) { ridA = rid[rA]; ridB = rid[rB]; }
     // 16-slot tiles that hold a real token (bit t = tile t).  An all-padding QUERY tile has dO = 0 (its rows are cropped
     // away): dS = 0 there, so it adds nothing to dQ / dK / dV / the bias gradients and both phases skip it.  (Padded
     // KEY tiles are kept: their dK / dV are part of the qkv-bias gradient.)
@@ -331,57 +355,72 @@ __global__ void __launch_bounds__(128, 3) window_attn_bwd7_kernel(
     const unsigned qvalid = ((b0 & 0xffffu) ? 1u : 0u) | ((b0 >> 16) ? 2u : 0u) | ((b1 & 0xffffu) ? 4u : 0u) | ((b1 >> 16) ? 8u : 0u);
     // ---------------- phase A: rows = queries ----------------
     if ((qvalid >> warp) & 1u) {
+      int ridA = 0, ridB = 0;
+      if (SHIFT) { ridA = rid[rA]; ridB = rid[rB]; }
+      // D = rowsum(dO * O) of rows rA / rB from the stored bf16 O: the four lanes of a row take 8 columns each
+      float DA = 0.f, DB = 0.f;
+      {
+        const int c8 = (lane & 3) * 8;
+        float fd[8], fo[8];
+        unpack8(*reinterpret_cast<const bf16x8*>(dOs + rA * LD + c8), fd);
+        unpack8(*reinterpret_cast<const bf16x8*>(Os + rA * LD + c8), fo);
+#pragma unroll
+        for (int j = 0; j < 8; j++) DA += fd[j] * fo[j];
+        unpack8(*reinterpret_cast<const bf16x8*>(dOs + rB * LD + c8), fd);
+        unpack8(*reinterpret_cast<const bf16x8*>(Os + rB * LD + c8), fo);
+#pragma unroll
+        for (int j = 0; j < 8; j++) DB += fd[j] * fo[j];
+        DA += __shfl_xor_sync(0xffffffffu, DA, 1);
+        DA += __shfl_xor_sync(0xffffffffu, DA, 2);
+        DB += __shfl_xor_sync(0xffffffffu, DB, 1);
+        DB += __shfl_xor_sync(0xffffffffu, DB, 2);
+      }
       uint32_t qa[2][4], da[2][4];
       ldsm_x4(qa[0], Qs + frag_off);
       ldsm_x4(qa[1], Qs + frag_off + 16);
       ldsm_x4(da[0], dOs + frag_off);
       ldsm_x4(da[1], dOs + frag_off + 16);
-      const float lA = Lraw[rA] * LOG2E, lB = Lraw[rB] * LOG2E, DA = Dsm[rA], DB = Dsm[rB];
+      const float lA = Lraw[rA] * LOG2E, lB = Lraw[rB] * LOG2E;
+#pragma unroll
+      for (int nt = 0; nt < C::NT8; nt++) {
+        float sacc[4] = {0.f, 0.f, 0.f, 0.f}, dp[4] = {0.f, 0.f, 0.f, 0.f};
+        uint32_t kb[4];
+        const int boff = (nt * 8 + (lane & 7)) * LD + (lane >> 3) * 8;
+        ldsm_x4(kb, Ks + boff);
+        mma16816(sacc, qa[0], kb[0], kb[1]);
+        mma16816(sacc, qa[1], kb[2], kb[3]);
+        ldsm_x4(kb, Vs + boff);
+        mma16816(dp, da[0], kb[0], kb[1]);
+        mma16816(dp, da[1], kb[2], kb[3]);
+        const int c0 = nt * 8 + (lane & 3) * 2;
+        float sv[4] = {fmaf(sacc[0], c, breg[nt][0]) - lA, fmaf(sacc[1], c, breg[nt][1]) - lA,
+                       fmaf(sacc[2], c, breg[nt][2]) - lB, fmaf(sacc[3], c, breg[nt][3]) - lB};
+        if (SHIFT) {
+          const int2 rc = *reinterpret_cast<const int2*>(rid + c0);
+          if (ridA != rc.x) sv[0] += -100.f * LOG2E;
+          if (ridA != rc.y) sv[1] += -100.f * LOG2E;
+          if (ridB != rc.x) sv[2] += -100.f * LOG2E;
+          if (ridB != rc.y) sv[3] += -100.f * LOG2E;
+        }
+        const float p[4] = {ex2(sv[0]), ex2(sv[1]), ex2(sv[2]), ex2(sv[3])};
+        const float ds[4] = {p[0] * (dp[0] - DA), p[1] * (dp[1] - DA), p[2] * (dp[2] - DB), p[3] * (dp[3] - DB)};
+#pragma unroll
+        for (int e = 0; e < 4; e++) dsacc[nt][e] += ds[e];
+        *reinterpret_cast<uint32_t*>(Ps + rA * PLD + c0) = pack_bf162(p[0], p[1]);
+        *reinterpret_cast<uint32_t*>(Ps + rB * PLD + c0) = pack_bf162(p[2], p[3]);
+        *reinterpret_cast<uint32_t*>(dSs + rA * PLD + c0) = pack_bf162(ds[0], ds[1]);
+        *reinterpret_cast<uint32_t*>(dSs + rB * PLD + c0) = pack_bf162(ds[2], ds[3]);
+      }
+      __syncwarp();  // this warp's rows of dS are in shared memory, and every lane has read its O rows
+      // dQ = dS K with dS read back as A fragments: the 16 accumulators are not live across the score loop
       float dq[4][4];
 #pragma unroll
       for (int dt = 0; dt < 4; dt++) dq[dt][0] = dq[dt][1] = dq[dt][2] = dq[dt][3] = 0.f;
 #pragma unroll
       for (int kk = 0; kk < 4; kk++) {
-        float ds2[2][4];
-#pragma unroll
-        for (int hf = 0; hf < 2; hf++) {
-          const int nt = 2 * kk + hf;
-          float sacc[4] = {0.f, 0.f, 0.f, 0.f};
-          ds2[hf][0] = ds2[hf][1] = ds2[hf][2] = ds2[hf][3] = 0.f;
-          uint32_t kb[4];
-          const int boff = (nt * 8 + (lane & 7)) * LD + (lane >> 3) * 8;
-          ldsm_x4(kb, Ks + boff);
-          mma16816(sacc, qa[0], kb[0], kb[1]);
-          mma16816(sacc, qa[1], kb[2], kb[3]);
-          ldsm_x4(kb, Vs + boff);
-          mma16816(ds2[hf], da[0], kb[0], kb[1]);
-          mma16816(ds2[hf], da[1], kb[2], kb[3]);
-          const int c0 = nt * 8 + (lane & 3) * 2;
-          const float2 bA = *reinterpret_cast<const float2*>(bm + rA * BLD + c0);
-          const float2 bB = *reinterpret_cast<const float2*>(bm + rB * BLD + c0);
-          float sv[4] = {fmaf(sacc[0], c, bA.x) - lA, fmaf(sacc[1], c, bA.y) - lA, fmaf(sacc[2], c, bB.x) - lB,
-                         fmaf(sacc[3], c, bB.y) - lB};
-          if (SHIFT) {
-            const int2 rc = *reinterpret_cast<const int2*>(rid + c0);
-            if (ridA != rc.x) sv[0] += -100.f * LOG2E;
-            if (ridA != rc.y) sv[1] += -100.f * LOG2E;
-            if (ridB != rc.x) sv[2] += -100.f * LOG2E;
-            if (ridB != rc.y) sv[3] += -100.f * LOG2E;
-          }
-          ds2[hf][0] = ex2(sv[0]) * (ds2[hf][0] - DA);
-          ds2[hf][1] = ex2(sv[1]) * (ds2[hf][1] - DA);
-          ds2[hf][2] = ex2(sv[2]) * (ds2[hf][2] - DB);
-          ds2[hf][3] = ex2(sv[3]) * (ds2[hf][3] - DB);
-#pragma unroll
-          for (int e = 0; e < 4; e++) dsacc[nt][e] += ds2[hf][e];
-        }
-        uint32_t sa[4];
-        sa[0] = pack_bf162(ds2[0][0], ds2[0][1]);
-        sa[1] = pack_bf162(ds2[0][2], ds2[0][3]);
-        sa[2] = pack_bf162(ds2[1][0], ds2[1][1]);
-        sa[3] = pack_bf162(ds2[1][2], ds2[1][3]);
+        uint32_t sa[4], kb[4];
+        ldsm_x4(sa, dSs + (r0 + (lane & 7) + ((lane >> 3) & 1) * 8) * PLD + kk * 16 + (lane >> 4) * 8);
         const bf16* kp = Ks + (kk * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * LD + (lane >> 4) * 8;
-        uint32_t kb[4];
         ldsm_x4_t(kb, kp);
         mma16816(dq[0], sa, kb[0], kb[1]);
         mma16816(dq[1], sa, kb[2], kb[3]);
@@ -389,23 +428,17 @@ __global__ void __launch_bounds__(128, 3) window_attn_bwd7_kernel(
         mma16816(dq[2], sa, kb[0], kb[1]);
         mma16816(dq[3], sa, kb[2], kb[3]);
       }
+      colsum_acc(dq, csum[0]);
 #pragma unroll
       for (int dt = 0; dt < 4; dt++) {
-        const int d = h * HD + dt * 8 + (lane & 3) * 2;
-        if (tA >= 0)
-          *reinterpret_cast<uint32_t*>(dqkv + (long long)tA * 3 * g.C + d) = pack_bf162(dq[dt][0] * scale, dq[dt][1] * scale);
-        if (tB >= 0)
-          *reinterpret_cast<uint32_t*>(dqkv + (long long)tB * 3 * g.C + d) = pack_bf162(dq[dt][2] * scale, dq[dt][3] * scale);
+        const int d = dt * 8 + (lane & 3) * 2;
+        *reinterpret_cast<uint32_t*>(Os + rA * LD + d) = pack_bf162(dq[dt][0] * scale, dq[dt][1] * scale);
+        *reinterpret_cast<uint32_t*>(Os + rB * LD + d) = pack_bf162(dq[dt][2] * scale, dq[dt][3] * scale);
       }
-      colsum_to_smem(dq, scale, dqb, lane);
     }
-    // ---------------- phase B: rows = keys (transposed recompute) ----------------
+    __syncthreads();  // P / dS complete; K and V are dead
+    // ---------------- phase B: rows = keys, P^T / dS^T read back transposed ----------------
     {
-      uint32_t ka[2][4], va[2][4];
-      ldsm_x4(ka[0], Ks + frag_off);
-      ldsm_x4(ka[1], Ks + frag_off + 16);
-      ldsm_x4(va[0], Vs + frag_off);
-      ldsm_x4(va[1], Vs + frag_off + 16);
       float dv[4][4], dk[4][4];
 #pragma unroll
       for (int dt = 0; dt < 4; dt++) {
@@ -415,50 +448,11 @@ __global__ void __launch_bounds__(128, 3) window_attn_bwd7_kernel(
 #pragma unroll
       for (int qq = 0; qq < 4; qq++) {
         if (!((qvalid >> qq) & 1u)) continue;
-        float pT[2][4], dsT[2][4];
-#pragma unroll
-        for (int hf = 0; hf < 2; hf++) {
-          const int nt = 2 * qq + hf;  // 8-query tile
-          pT[hf][0] = pT[hf][1] = pT[hf][2] = pT[hf][3] = 0.f;
-          dsT[hf][0] = dsT[hf][1] = dsT[hf][2] = dsT[hf][3] = 0.f;
-          uint32_t qb[4];
-          const int boff = (nt * 8 + (lane & 7)) * LD + (lane >> 3) * 8;
-          ldsm_x4(qb, Qs + boff);
-          mma16816(pT[hf], ka[0], qb[0], qb[1]);
-          mma16816(pT[hf], ka[1], qb[2], qb[3]);
-          ldsm_x4(qb, dOs + boff);
-          mma16816(dsT[hf], va[0], qb[0], qb[1]);
-          mma16816(dsT[hf], va[1], qb[2], qb[3]);
-          const int q0 = nt * 8 + (lane & 3) * 2;  // the two query columns of this thread
-          const float2 lq = *reinterpret_cast<const float2*>(Lraw + q0);
-          const float2 Dq = *reinterpret_cast<const float2*>(Dsm + q0);
-          // bias[query][key]: rows q0, q0+1 of the table, columns = this thread's key rows
-          float sv[4] = {fmaf(pT[hf][0], c, bm[q0 * BLD + rA]) - lq.x * LOG2E,
-                         fmaf(pT[hf][1], c, bm[(q0 + 1) * BLD + rA]) - lq.y * LOG2E,
-                         fmaf(pT[hf][2], c, bm[q0 * BLD + rB]) - lq.x * LOG2E,
-                         fmaf(pT[hf][3], c, bm[(q0 + 1) * BLD + rB]) - lq.y * LOG2E};
-          if (SHIFT) {
-            const int2 rq = *reinterpret_cast<const int2*>(rid + q0);
-            if (ridA != rq.x) sv[0] += -100.f * LOG2E;
-            if (ridA != rq.y) sv[1] += -100.f * LOG2E;
-            if (ridB != rq.x) sv[2] += -100.f * LOG2E;
-            if (ridB != rq.y) sv[3] += -100.f * LOG2E;
-          }
-          pT[hf][0] = ex2(sv[0]); pT[hf][1] = ex2(sv[1]); pT[hf][2] = ex2(sv[2]); pT[hf][3] = ex2(sv[3]);
-          dsT[hf][0] = pT[hf][0] * (dsT[hf][0] - Dq.x);
-          dsT[hf][1] = pT[hf][1] * (dsT[hf][1] - Dq.y);
-          dsT[hf][2] = pT[hf][2] * (dsT[hf][2] - Dq.x);
-          dsT[hf][3] = pT[hf][3] * (dsT[hf][3] - Dq.y);
-        }
+        // A fragments (16 keys x 16 queries) of the transposes: matrix j of the x4 load = queries +8 (j >> 1), keys +8 (j & 1)
+        const int aoff = (qq * 16 + (lane >> 4) * 8 + (lane & 7)) * PLD + r0 + ((lane >> 3) & 1) * 8;
         uint32_t pa[4], sa[4];
-        pa[0] = pack_bf162(pT[0][0], pT[0][1]);
-        pa[1] = pack_bf162(pT[0][2], pT[0][3]);
-        pa[2] = pack_bf162(pT[1][0], pT[1][1]);
-        pa[3] = pack_bf162(pT[1][2], pT[1][3]);
-        sa[0] = pack_bf162(dsT[0][0], dsT[0][1]);
-        sa[1] = pack_bf162(dsT[0][2], dsT[0][3]);
-        sa[2] = pack_bf162(dsT[1][0], dsT[1][1]);
-        sa[3] = pack_bf162(dsT[1][2], dsT[1][3]);
+        ldsm_x4_t(pa, Ps + aoff);
+        ldsm_x4_t(sa, dSs + aoff);
         const int toff = (qq * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * LD + (lane >> 4) * 8;
         uint32_t bb[4];
         ldsm_x4_t(bb, dOs + toff);
@@ -474,24 +468,40 @@ __global__ void __launch_bounds__(128, 3) window_attn_bwd7_kernel(
         mma16816(dk[2], sa, bb[0], bb[1]);
         mma16816(dk[3], sa, bb[2], bb[3]);
       }
+      colsum_acc(dk, csum[1]);
 #pragma unroll
       for (int dt = 0; dt < 4; dt++) {
-        const int d = h * HD + dt * 8 + (lane & 3) * 2;
-        if (tA >= 0) {
-          bf16* base = dqkv + (long long)tA * 3 * g.C + d;
-          *reinterpret_cast<uint32_t*>(base + g.C) = pack_bf162(dk[dt][0] * scale, dk[dt][1] * scale);
-          *reinterpret_cast<uint32_t*>(base + 2 * g.C) = pack_bf162(dv[dt][0], dv[dt][1]);
-        }
-        if (tB >= 0) {
-          bf16* base = dqkv + (long long)tB * 3 * g.C + d;
-          *reinterpret_cast<uint32_t*>(base + g.C) = pack_bf162(dk[dt][2] * scale, dk[dt][3] * scale);
-          *reinterpret_cast<uint32_t*>(base + 2 * g.C) = pack_bf162(dv[dt][2], dv[dt][3]);
+        vsum[2 * dt * NTHREADS] += dv[dt][0] + dv[dt][2];
+        vsum[(2 * dt + 1) * NTHREADS] += dv[dt][1] + dv[dt][3];
+      }
+#pragma unroll
+      for (int dt = 0; dt < 4; dt++) {
+        const int d = dt * 8 + (lane & 3) * 2;
+        *reinterpret_cast<uint32_t*>(Ks + rA * LD + d) = pack_bf162(dk[dt][0] * scale, dk[dt][1] * scale);
+        *reinterpret_cast<uint32_t*>(Ks + rB * LD + d) = pack_bf162(dk[dt][2] * scale, dk[dt][3] * scale);
+        *reinterpret_cast<uint32_t*>(Vs + rA * LD + d) = pack_bf162(dv[dt][0], dv[dt][1]);
+        *reinterpret_cast<uint32_t*>(Vs + rB * LD + d) = pack_bf162(dv[dt][2], dv[dt][3]);
+      }
+    }
+    __syncthreads();  // dQ / dK / dV staged; nobody reads Q / dO / P / dS of this item any more
+    // A thread stores the (slot, 16-byte chunk) pairs that it gathers in issue7, so the next gather into this stage
+    // needs no further block barrier: it overwrites only what the same thread has read.
+    {
+      const int c16 = threadIdx.x & 3;
+#pragma unroll
+      for (int kk = 0; kk < 256 / NTHREADS; kk++) {
+        const int t = (threadIdx.x >> 2) + (NTHREADS / 4) * kk;
+        const int tk = tok[t];
+        if (tk >= 0) {
+          bf16* dst = dqkv + (long long)tk * 3 * g.C + h * HD + c16 * 8;
+          const int so = t * LD + c16 * 8;
+          *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(Os + so);
+          *reinterpret_cast<uint4*>(dst + g.C) = *reinterpret_cast<const uint4*>(Ks + so);
+          *reinterpret_cast<uint4*>(dst + 2 * g.C) = *reinterpret_cast<const uint4*>(Vs + so);
         }
       }
-      colsum_to_smem(dk, scale, dqb + HD, lane);
-      colsum_to_smem(dv, 1.f, dqb + 2 * HD, lane);
+      __syncwarp();  // tok of this stage is rewritten by the first lane of each quad
     }
-    __syncthreads();  // stage (and Dsm) free for the next-but-one gather
   }
   cp_async_wait<0>();
   // flush the register-resident rel-pos-bias gradient of this warp's query rows.  dS was formed with the true
@@ -504,6 +514,16 @@ __global__ void __launch_bounds__(128, 3) window_attn_bwd7_kernel(
       const int col = nt * 8 + (lane & 3) * 2 + (e & 1);
       if (row < C::NT && col < C::NT) atomicAdd(&dbt[bias_index<WS>(row, col)], dsacc[nt][e]);
     }
+  // and the qkv-bias gradient: sum over the 8 row groups of the warp, then over the warps
+#pragma unroll
+  for (int part = 0; part < 3; part++)
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+      float v = part < 2 ? csum[part][i] : vsum[i * NTHREADS];
+#pragma unroll
+      for (int o = 4; o < 32; o <<= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      if (lane < 4) atomicAdd(&dqb[part * HD + (i >> 1) * 8 + lane * 2 + (i & 1)], part < 2 ? v * scale : v);
+    }
   __syncthreads();
   for (int i = threadIdx.x; i < C::NB; i += NTHREADS) atomicAdd(&dbias_table[i * g.nH + h], dbt[i]);
   for (int i = threadIdx.x; i < 3 * HD; i += NTHREADS)
@@ -512,7 +532,8 @@ __global__ void __launch_bounds__(128, 3) window_attn_bwd7_kernel(
 
 static size_t bwd7_smem() {
   using C = Cfg<7>;
-  return (size_t)2 * 5 * TILE7 * 2 + (size_t)(C::KP * BLD + C::NB + 1 + 3 * HD + C::KP + 2 * 64) * 4 + (size_t)4 * 64 * 4;
+  return (size_t)2 * 5 * TILE7 * 2 + (size_t)2 * C::KP * PLD * 2 + (size_t)(C::NB + 3 + 3 * HD + 2 * 64) * 4 + (size_t)4 * 64 * 4 +
+         (size_t)3 * 4 * 16 + (size_t)8 * 128 * 4;
 }
 
 }  // namespace wa
