@@ -23,8 +23,8 @@ import torch
 import torch.distributed as dist
 import torch.nn as nn
 
-from . import linear, ops
-from .swin_transformer import _CastCache
+from . import backbone, linear, ops
+from .backbone import MultiCropBackbone, _CastCache
 
 Tensor = torch.Tensor
 BF16 = torch.bfloat16
@@ -127,19 +127,16 @@ class Transformer(nn.Module):
                                   kernel_size=kernel_qkv, padding=padding_qkv, window_size=window_size, shift_size=0,
                                   rel_pos_embed=rel_pos_embed)),
                 PreNorm(norm_layer, embed_dim, FeedForward(embed_dim, act_layer, mlp_ratio)),
-                nn.Identity(),  # DropPath: parameter-free; the per-row scales are drawn by CvT._stage_keeps
+                nn.Identity(),  # DropPath: parameter-free; the per-row scales are drawn by CvT._run
             ]))
         self.window_size = window_size
         self.shift = shift
 
     def block(self, j: int, x: Tensor, pend, wgroups, cc: _CastCache, k1: Optional[Tensor], k2: Optional[Tensor]):
-        """(x fp32 [T, C], pending MLP delta) -> (x, pending) of layer j (:333-335)"""
+        """backbone.pre_norm_block of layer j (:333-335)"""
         attn, ff, _ = self.layers[j]
-        delta, keep, dbias = pend if pend is not None else (None, None, None)
-        x, y = ops.add_layer_norm(x, delta, keep, attn.norm.weight, attn.norm.bias, attn.norm.eps, delta_bias=dbias)
-        a = attn.fn.fused(y, wgroups, cc)
-        x, y = ops.add_layer_norm(x, a, k1, ff.norm.weight, ff.norm.bias, ff.norm.eps, delta_bias=attn.fn.proj_out.bias)
-        return x, (ff.fn.fused(y, cc), k2, ff.fn.net[2].bias)
+        return backbone.pre_norm_block(x, pend, attn.norm, lambda y: attn.fn.fused(y, wgroups, cc), ff.norm,
+                                       attn.fn.proj_out.bias, lambda y: ff.fn.fused(y, cc), ff.fn.net[2].bias, k1, k2)
 
 
 class ConvEmbed(nn.Module):
@@ -181,7 +178,7 @@ def _spec(spec, key, default=None):
     return getattr(spec, key, default)
 
 
-class CvT(nn.Module):
+class CvT(MultiCropBackbone):
     """:434-661"""
 
     def __init__(self, *, num_classes, act_layer=nn.GELU, norm_layer=nn.LayerNorm, init='trunc_norm',
@@ -251,9 +248,7 @@ class CvT(nn.Module):
 
     def _geometry(self, imgs: Sequence[Tensor]):
         """per stage: (token groups ((B, H, W, row0), ...), window groups ((B, H, W, w, row0, prow0), ...))"""
-        for im in imgs:
-            if im.dim() != 4 or im.shape[1] != 3:
-                raise ValueError(f"expected crops [B, 3, H, W], got {tuple(im.shape)}")
+        backbone.check_crops(imgs)
         sizes = [(im.shape[0], im.shape[2], im.shape[3]) for im in imgs]
         geo = []
         for i in range(self.num_stages):
@@ -273,35 +268,15 @@ class CvT(nn.Module):
             geo.append((tuple(tg), tuple(wg)))
         return geo
 
-    def _stage_keeps(self, i: int, tg, device) -> Optional[Tensor]:
-        """per-row DropPath scales fp32 [2 * depth, T] of stage i (timm: floor(keep_prob + U) / keep_prob per (call,
-        sample)), drawn by one torch.rand; None when no block of the stage drops"""
-        tr = self._stage(i)[1]
-        if not self.training or not any(p > 0. for p in tr.drop_probs):
-            return None
-        # the keep probabilities and the row -> image map are built once per geometry (eagerly, before a CUDA-graph
-        # capture replays the step): no host-to-device copy inside the step
-        cache = self.__dict__.setdefault("_keep_cache", {})
-        key = (i, tg, device)
-        ent = cache.get(key)
-        if ent is None:
-            if len(cache) >= 32:   # a handful of crop geometries per run
-                cache.clear()
-            kp = torch.tensor([[1.0 - p] for p in tr.drop_probs for _ in range(2)], dtype=torch.float32).to(device)
-            rs = torch.arange(sum(B for B, _, _, _ in tg), device=device).repeat_interleave(
-                torch.tensor([H * W for B, H, W, _ in tg for _ in range(B)], device=device))
-            ent = cache[key] = (kp, rs)
-        kp, rs = ent
-        nb = sum(B for B, _, _, _ in tg)
-        r = torch.rand(kp.shape[0], nb, dtype=torch.float32, device=device)
-        return r.add_(kp).floor_().div_(kp).index_select(1, rs)
+    def _depths(self) -> List[int]:
+        return [len(self._stage(i)[1].layers) for i in range(self.num_stages)]
 
     def _run(self, imgs: List[Tensor], taps=None):
-        """-> (stream fp32 [T, C] after the last stage, pending delta, last-stage token groups); taps(i, j, x) is called
-        with the materialised output of every block (i, j) it returns True for (forward_return_n_last_blocks)."""
+        """-> (stream fp32 [T, C] after the last stage, pending delta, last-stage token groups); taps: see backbone.tap,
+        called with the stage's token groups."""
         cc = _CastCache()
         geo = self._geometry(imgs)
-        x, pend, prev = None, None, None
+        x, pend, prev, b = None, None, None, 0
         for i in range(self.num_stages):
             emb, tr = self._stage(i)
             tg, wg = geo[i]
@@ -310,76 +285,28 @@ class CvT(nn.Module):
             else:
                 x = emb.fused(ops.residual_add(x, *pend) if pend is not None else x, prev, cc)
             pend = None
-            keeps = self._stage_keeps(i, tg, x.device)
+            probs = [p for p in tr.drop_probs for _ in range(2)]
+            scales = backbone.drop_path_scales(self, probs, sum(B for B, _, _, _ in tg), x.device)
+            keeps = backbone.drop_path_rows(self, scales, [(B, H * W) for B, H, W, _ in tg], x.device)
             for j in range(len(tr.layers)):
                 k1 = k2 = None
                 if keeps is not None and tr.drop_probs[j] > 0.:
                     k1, k2 = keeps[2 * j], keeps[2 * j + 1]
                 x, pend = tr.block(j, x, pend, wg, cc, k1, k2)
-                if taps is not None and taps(i, j):
-                    x, pend = ops.residual_add(x, *pend), None
-                    taps.out.append(self._tap_feature(i, x, tg))
+                x, pend = backbone.tap(taps, b, x, pend, tg)
+                b += 1
             prev = tg
         return x, pend, geo[-1][0]
 
     def _tap_feature(self, i: int, x: Tensor, tg) -> Tensor:
-        if i == self.num_stages - 1:  # :602-605 the final norm on the last stage's blocks
-            x = ops.LayerNormFn.apply(x, self.norm.weight, self.norm.bias, self.norm.eps, False)
+        """:567-615: the token mean of a block's output"""
         return ops.TokenMeanGroupsFn.apply(x, tg)
 
-    def _features(self, imgs: List[Tensor]):
-        """-> (pooled fp32 [sum B, C], region fp32 [sum B*N, C] = the final norm's tokens, token groups)"""
-        x, pend, tg = self._run(imgs)
-        delta, keep, dbias = pend if pend is not None else (None, None, None)
-        _, region = ops.add_layer_norm(x, delta, keep, self.norm.weight, self.norm.bias, self.norm.eps, y_bf16=False,
-                                       delta_bias=dbias)
-        return ops.TokenMeanGroupsFn.apply(region, tg), region, tg
-
-    def forward_features(self, x: Tensor):
-        """:549-563 -> pooled fp32 [B, C] (and the normed region tokens fp32 [B, N, C] in dense mode)"""
-        pooled, region, tg = self._features([x.float()])
-        if self.use_dense_prediction:
-            B, H, W, _ = tg[0]
-            return pooled, region.view(B, H * W, -1)
-        return pooled
-
-    def forward_return_n_last_blocks(self, x: Tensor, n: int = 1, return_patch_avgpool: bool = False, depth=[]):
-        """:567-615 (eval_linear.py's probe features): the token mean of each of the last n blocks' outputs (the last
-        stage's through the final norm), concatenated.  `depth` lists the blocks per stage as in the reference;
-        return_patch_avgpool is ignored, as there."""
-        depths = [len(self._stage(i)[1].layers) for i in range(self.num_stages)]
-        if list(depth) != depths:
-            raise ValueError(f"depth must list the blocks per stage {depths}, got {list(depth)}")
-        if not 1 <= int(n) <= sum(depths):
-            raise ValueError(f"n must be in [1, {sum(depths)}], got {n}")
-        start = sum(depths) - int(n)
-        first = {}
-        acc = 0
-        for i, d in enumerate(depths):
-            first[i] = acc
-            acc += d
-
-        def taps(i, j):
-            return first[i] + j >= start
-
-        taps.out = []
-        self._run([x.float()], taps)
-        return torch.cat(taps.out, dim=-1)
-
-    def forward(self, x):
-        """Multi-crop forward (:619-661): consecutive same-resolution crops form one group; the outputs are concatenated
-        group-major exactly as the reference's per-group loop concatenates them."""
-        if not isinstance(x, list):
-            x = [x]
-        groups, start = [], 0
-        for i in range(1, len(x) + 1):
-            if i == len(x) or x[i].shape[-1] != x[start].shape[-1]:
-                groups.append((start, i))
-                start = i
-        pooled, region, tg = self._features([ops.cat_adjacent(x[s:e]).float() for s, e in groups])
-        if self.use_dense_prediction:
-            return self.head(pooled), self.head_dense(region), region, [H * W for _, H, W, _ in tg]
-        return self.head(pooled)
+    def _features(self, imgs: List[Tensor], taps=None):
+        """-> (pooled fp32 [sum B, C], region fp32 [sum B*N, C] = the final norm's tokens, tokens per image)"""
+        x, pend, tg = self._run(imgs, taps)
+        region = self._final_norm(x, pend)
+        return ops.TokenMeanGroupsFn.apply(region, tg), region, [H * W for _, H, W, _ in tg]
 
 
 def get_cls_model(config, is_teacher=False, use_dense_prediction=False, **kwargs):

@@ -22,13 +22,14 @@ from __future__ import annotations
 import math
 import os
 from functools import partial
-from typing import Dict, List, Optional, Sequence
+from typing import List, Optional, Sequence
 
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import linear, ops, shadow
+from . import backbone, linear, ops, shadow
+from .backbone import MultiCropBackbone, _CastCache
 
 Tensor = torch.Tensor
 BF16 = torch.bfloat16
@@ -51,44 +52,6 @@ def _lin(x: Tensor, w: Tensor, b: Optional[Tensor]) -> Tensor:
         return F.linear(x, w.to(BF16), None if b is None else b.to(BF16))
 
 
-class _CastCache:
-    """bf16 copies of weights shared by the resolution groups of one forward call (one cast per step)."""
-
-    def __init__(self):
-        self.d: Dict[int, Tensor] = {}
-
-    def __call__(self, p: Optional[Tensor]) -> Optional[Tensor]:
-        if p is None:
-            return None
-        k = id(p)
-        t = self.d.get(k)
-        if t is None:
-            t = self.d[k] = shadow.as_bf16(p)  # optimiser-maintained bf16 shadow when registered, else a cast
-        return t
-
-    def transposed(self, p: Tensor) -> Tensor:
-        """bf16 W^T (contiguous) of a 2-D weight: the K-major operand of the fused input-gradient GEMM (ops.MlpFn)."""
-        k = ("T", id(p))
-        t = self.d.get(k)
-        if t is None:
-            t = self.d[k] = shadow.as_bf16(p, track_grad=False).t().contiguous()
-        return t
-
-    def expanded_bias(self, table: Tensor, num_heads: int, ws: int) -> Optional[Tensor]:
-        """the rel-pos bias table expanded once per forward call (ops.expand_rel_pos_bias), shared by the crop groups."""
-        k = ("B", id(table))
-        if k not in self.d:
-            self.d[k] = ops.expand_rel_pos_bias(table, num_heads, ws)
-        return self.d[k]
-
-    def nograd(self, p: Tensor) -> Tensor:
-        k = ("ng", id(p))
-        t = self.d.get(k)
-        if t is None:
-            t = self.d[k] = shadow.as_bf16(p, track_grad=False)
-        return t
-
-
 def _lin_c(x: Tensor, lin: nn.Linear, cc: Optional[_CastCache]) -> Tensor:
     """bf16 library GEMM x @ W^T + b (bias in the GEMM epilogue).  The bias GRADIENT is not computed here: the consumer
     kernel (window attention / GELU / residual add + LN backward) column-sums it, see ops.LinearBiasFn."""
@@ -100,15 +63,6 @@ def _lin_c(x: Tensor, lin: nn.Linear, cc: Optional[_CastCache]) -> Tensor:
         with torch.autocast("cuda", enabled=False):
             return F.linear(x, w)
     return ops.LinearBiasFn.apply(x, w, (shadow.as_bf16(lin.bias, False) if cc is None else cc.nograd(lin.bias)))
-
-
-def drop_path_keep(batch: int, drop_prob: float, training: bool, device) -> Optional[Tensor]:
-    """Per-sample stochastic-depth scale (0 or 1/keep_prob) of timm 0.3.2 DropPath; None = identity."""
-    if drop_prob == 0. or not training:
-        return None
-    keep_prob = 1.0 - drop_prob
-    r = keep_prob + torch.rand(batch, dtype=torch.float32, device=device)
-    return r.floor_().div_(keep_prob)
 
 
 def _one_group(x: Tensor):
@@ -225,28 +179,16 @@ class SwinTransformerBlock(nn.Module):
 
     def fused(self, x: Optional[Tensor], pending, grp, cc: Optional[_CastCache], k1: Optional[Tensor],
               k2: Optional[Tensor], maps: Optional[List[Tensor]] = None):
-        """(x fp32 [T, C] of the resolution groups grp = ((B, H, W, row0), ...), pending = (delta bf16, keep,
-        delta_bias) or None) -> (x, pending): the MLP branch's residual add (and fc2 bias) is deferred into the next
-        fused add+LN.  x None: the stream starts as fp32(delta) (after PatchMerging).  k1 / k2: per-ROW DropPath
-        scales (fp32 [T]) or None.  maps: see WindowAttention.attend."""
-        delta, keep, dbias = pending if pending is not None else (None, None, None)
-        x, y = ops.add_layer_norm(x, delta, keep, self.norm1.weight, self.norm1.bias, self.norm1.eps, delta_bias=dbias)
-        a = self.attn.attend(y, grp, self.shift_size, cc, maps)
-        x, y = ops.add_layer_norm(x, a, k1, self.norm2.weight, self.norm2.bias, self.norm2.eps,
-                                  delta_bias=self.attn.proj.bias)
-        z = self.mlp.fused(y, cc)
-        return x, (z, k2, self.mlp.fc2.bias)
-
-    def keeps(self, B: int, L: int, device) -> List[Optional[Tensor]]:
-        """[k1, k2]: the two DropPath scales of a call on B samples of L tokens outside the backbone, drawn per sample
-        (drop_path_keep) and spread per row (fp32 [B*L]); None = identity."""
-        ks = [drop_path_keep(B, self.drop_prob, self.training, device) for _ in range(2)]
-        return [None if k is None else k.repeat_interleave(L) for k in ks]
+        """backbone.pre_norm_block over the resolution groups grp = ((B, H, W, row0), ...); x None: the stream starts
+        after PatchMerging.  maps: see WindowAttention.attend."""
+        return backbone.pre_norm_block(x, pending, self.norm1,
+                                       lambda y: self.attn.attend(y, grp, self.shift_size, cc, maps), self.norm2,
+                                       self.attn.proj.bias, lambda y: self.mlp.fused(y, cc), self.mlp.fc2.bias, k1, k2)
 
     def forward(self, x: Tensor):
         """Reference signature: x [B, L, C] -> (x, attn); attn probabilities are not materialised (None)."""
         xs, grp = _one_group(x.float())
-        xs, pend = self.fused(xs, None, grp, None, *self.keeps(x.shape[0], x.shape[1], x.device))
+        xs, pend = self.fused(xs, None, grp, None, *backbone.block_keeps(self, x.shape[0], x.shape[1], x.device))
         return ops.residual_add(xs, *pend).view(x.shape), None
 
 
@@ -296,16 +238,13 @@ class BasicLayer(nn.Module):
         the downsample).  After a downsample the stream is handed on as (None, (merged bf16, None, None)): the next
         stage's first add+LN turns it into the fp32 residual.  keeps: per-row DropPath scales [2*depth][T] of this
         layer or None.  Per block j: maps[j] is the list its attention probabilities are appended to, or None;
-        taps[j], if not None, makes the block's output materialise (residual_add) and is called with it and grp, and
-        the stream continues from it."""
+        taps: see backbone.tap, called with grp."""
         for j, blk in enumerate(self.blocks):
             k1 = k2 = None
             if keeps is not None and blk.drop_prob > 0. and blk.training:
                 k1, k2 = keeps[2 * j], keeps[2 * j + 1]
             x, pend = blk.fused(x, pend, grp, cc, k1, k2, None if maps is None else maps[j])
-            if taps is not None and taps[j] is not None:
-                x, pend = ops.residual_add(x, *pend), None
-                taps[j](x, grp)
+            x, pend = backbone.tap(taps, j, x, pend, grp)
         if self.downsample is not None:
             if pend is not None:
                 x = ops.residual_add(x, *pend)
@@ -316,7 +255,7 @@ class BasicLayer(nn.Module):
     def _forward(self, x: Tensor, maps=None, taps=None) -> Tensor:
         """x [B, L, C] as one group through fused() -> fp32 [B, L', C'] after the downsample"""
         B, L, _ = x.shape
-        keeps = [k for blk in self.blocks for k in blk.keeps(B, L, x.device)]
+        keeps = [k for blk in self.blocks for k in backbone.block_keeps(blk, B, L, x.device)]
         xs, grp = _one_group(x.float())
         xs, pend, _ = self.fused(xs, None, grp, None, keeps, maps, taps)
         if xs is None:  # after the downsample: the merged bf16 tokens
@@ -374,7 +313,7 @@ class PatchEmbed(nn.Module):
         return xs.view(x.shape[0], -1, xs.shape[-1])
 
 
-class SwinTransformer(nn.Module):
+class SwinTransformer(MultiCropBackbone):
     def __init__(self, img_size=224, patch_size=4, in_chans=3, num_classes=1000, embed_dim=96, depths=[2, 2, 6, 2],
                  num_heads=[3, 6, 12, 24], window_size=7, mlp_ratio=4., qkv_bias=True, qk_scale=None, drop_rate=0.,
                  attn_drop_rate=0., drop_path_rate=0.1, norm_layer=nn.LayerNorm, ape=False, patch_norm=True,
@@ -425,29 +364,8 @@ class SwinTransformer(nn.Module):
     def no_weight_decay_keywords(self):
         return {'relative_position_bias_table'}
 
-    def _row_samples(self, grp, device) -> Tensor:
-        """int64 [T]: the (global) sample index of every token row of the concatenated groups (cached per geometry)."""
-        cache = self.__dict__.setdefault("_rs_cache", {})
-        key = (tuple(grp), device)
-        t = cache.get(key)
-        if t is None:
-            if len(cache) >= 32:  # a handful of crop geometries per run; keep the cache from growing with odd batches
-                cache.clear()
-            parts, b0 = [], 0
-            for B, H, W, _ in grp:
-                parts.append(torch.arange(b0, b0 + B, device=device).repeat_interleave(H * W))
-                b0 += B
-            t = cache[key] = torch.cat(parts)
-        return t
-
-    def _keep_prob_column(self, device) -> Tensor:
-        """device fp32 [2*nblk, 1] of 1 - drop_prob (two DropPath calls per block), built once per device."""
-        cache = self.__dict__.setdefault("_kp_cache", {})
-        t = cache.get(device)
-        if t is None:
-            probs = [[1.0 - blk.drop_prob] for layer in self.layers for blk in layer.blocks for _ in range(2)]
-            t = cache[device] = torch.tensor(probs, dtype=torch.float32).to(device)
-        return t
+    def _depths(self) -> List[int]:
+        return [len(layer.blocks) for layer in self.layers]
 
     def _run(self, x, taps=None, maps=None):
         """The backbone with ONE pass over the concatenated tokens of all resolution groups for every per-token op (same
@@ -458,61 +376,27 @@ class SwinTransformer(nn.Module):
         cc = _CastCache()
         x, grp = _one_group(x) if isinstance(x, Tensor) else self.patch_embed.fused(x)
         dev = x.device
-        keeps_all = None
-        if self.training and any(blk.drop_prob > 0. for layer in self.layers for blk in layer.blocks):
-            kp = self._keep_prob_column(dev)                                    # [2*nblk, 1]
-            r = torch.rand(kp.shape[0], sum(g[0] for g in grp), dtype=torch.float32, device=dev)
-            keeps_all = r.add_(kp).floor_().div_(kp)                            # timm DropPath scale per (call, sample)
+        probs = [blk.drop_prob for layer in self.layers for blk in layer.blocks for _ in range(2)]
+        scales = backbone.drop_path_scales(self, probs, sum(g[0] for g in grp), dev)
         pend, b = None, 0
         for layer in self.layers:
             d = len(layer.blocks)
-            keeps = None
-            if keeps_all is not None:
-                keeps = keeps_all[2 * b:2 * (b + d)].index_select(1, self._row_samples(grp, dev))
+            keeps = backbone.drop_path_rows(self, None if scales is None else scales[2 * b:2 * (b + d)],
+                                            [(B, H * W) for B, H, W, _ in grp], dev)
             x, pend, grp = layer.fused(x, pend, grp, cc, keeps, None if maps is None else maps[b:b + d],
                                        None if taps is None else taps[b:b + d])
             b += d
         return x, pend, grp
 
     def _features(self, imgs: List[Tensor], taps=None):
-        """-> (pooled fp32 [sum B, D], region fp32 [T, D] = the final norm's tokens, the last stage's grp)"""
+        """-> (pooled fp32 [sum B, D], region fp32 [T, D] = the final norm's tokens, tokens per image of each group)"""
         x, pend, grp = self._run(imgs, taps)
-        delta, keep, dbias = pend if pend is not None else (None, None, None)
-        _, region = ops.add_layer_norm(x, delta, keep, self.norm.weight, self.norm.bias, self.norm.eps,
-                                       y_bf16=False, delta_bias=dbias)
-        return ops.TokenMeanGroupsFn.apply(region, tuple(grp)), region, grp
+        region = self._final_norm(x, pend)
+        return ops.TokenMeanGroupsFn.apply(region, tuple(grp)), region, [H * W for _, H, W, _ in grp]
 
-    def forward_features(self, x: Tensor):
-        """models/swin_transformer.py:678-694 -> pooled fp32 [B, D] (and region fp32 [B, N, D] in dense mode)."""
-        pooled, region, _ = self._features([x.float()])
-        if self.use_dense_prediction:
-            return pooled, region.view(x.shape[0], -1, region.shape[-1])
-        return pooled
-
-    def forward_return_n_last_blocks(self, x: Tensor, n: int = 1, return_patch_avgpool: bool = False, depth=[]):
-        """models/swin_transformer.py:799-837 (eval_linear.py's probe features): fp32 [B, sum C_i], the token means of
-        the outputs of the last n blocks in execution order; outputs of last-stage blocks go through the final norm
-        first.  return_patch_avgpool is ignored, as in the reference.  `depth` must equal the model's depths.
-
-        Only a tapped block's output is materialised (residual_add), and the stream continues from it; the last
-        block's normed output is the final add+LN output itself."""
-        depths = [len(layer.blocks) for layer in self.layers]
-        if [int(d) for d in depth] != depths:
-            raise ValueError(f"depth {list(depth)} does not match the model's depths {depths}")
-        total = sum(depths)
-        if not 1 <= int(n) <= total:
-            raise ValueError(f"n must be in [1, {total}], got {n}")
-        start, last = total - int(n), len(self.layers) - 1
-        out = []
-
-        def tap(normed: bool, x: Tensor, grp):
-            y = ops.LayerNormFn.apply(x, self.norm.weight, self.norm.bias, self.norm.eps, False) if normed else x
-            out.append(ops.TokenMeanGroupsFn.apply(y, tuple(grp)))
-
-        taps = [partial(tap, i == last) for i, d in enumerate(depths) for _ in range(d)]
-        taps = [t if start <= b < total - 1 else None for b, t in enumerate(taps)]
-        pooled, _, _ = self._features([x.float()], taps)
-        return torch.cat(out + [pooled], dim=-1)
+    def _tap_feature(self, i: int, x: Tensor, grp) -> Tensor:
+        """models/swin_transformer.py:799-837: the token mean of a block's output"""
+        return ops.TokenMeanGroupsFn.apply(x, tuple(grp))
 
     def _attention_maps(self, x, last: bool):
         """_run's input -> the last block's attention probabilities (last) or every block's in execution order; only
@@ -556,21 +440,6 @@ class SwinTransformer(nn.Module):
             return self.forward_features(x)
         finally:
             self.use_dense_prediction = d
-
-    def forward(self, x):
-        """Multi-crop forward (models/swin_transformer.py:713-763): consecutive same-resolution crops form one group; the
-        outputs are concatenated group-major exactly as the reference's per-group loop concatenates them."""
-        if not isinstance(x, list):
-            x = [x]
-        groups, start = [], 0
-        for i in range(1, len(x) + 1):
-            if i == len(x) or x[i].shape[-1] != x[start].shape[-1]:
-                groups.append((start, i))
-                start = i
-        pooled, region, grp = self._features([ops.cat_adjacent(x[s:e]).float() for s, e in groups])
-        if self.use_dense_prediction:
-            return self.head(pooled), self.head_dense(region), region, [H * W for _, H, W, _ in grp]
-        return self.head(pooled)
 
 
 def get_cls_model(config, is_teacher=False, use_dense_prediction=False, **kwargs):

@@ -27,8 +27,8 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import linear, ops
-from .swin_transformer import _CastCache
+from . import backbone, linear, ops
+from .backbone import MultiCropBackbone, _CastCache
 
 Tensor = torch.Tensor
 BF16 = torch.bfloat16
@@ -408,7 +408,7 @@ class MlpBlock(nn.Module):
         self.shortcut = nn.Identity()
 
 
-class MsViT(nn.Module):
+class MsViT(MultiCropBackbone):
     """:406-769"""
 
     def __init__(self, arch, img_size=512, in_chans=3, num_classes=1000, qkv_bias=True, qk_scale=None, drop_rate=0.,
@@ -570,9 +570,7 @@ class MsViT(nn.Module):
 
     def _geometry(self, imgs: Sequence[Tensor]):
         """per stage: ((B, H, W, N, row0), ...) with N = Nglo + H*W rows per image"""
-        for im in imgs:
-            if im.dim() != 4 or im.shape[1] != 3:
-                raise ValueError(f"expected crops [B, 3, H, W], got {tuple(im.shape)}")
+        backbone.check_crops(imgs)
         sizes = [(im.shape[0], im.shape[2], im.shape[3]) for im in imgs]
         geo = []
         for i, cfg in enumerate(self.layer_cfgs):
@@ -588,34 +586,17 @@ class MsViT(nn.Module):
             geo.append(tuple(st))
         return geo
 
-    def _stage_keeps(self, i: int, st, device) -> Optional[Tensor]:
-        """per-row DropPath scales fp32 [2 * blocks, T] of stage i (AttnBlock, MlpBlock of every block; timm: floor(keep
-        + U) / keep per (call, image), the global row included), drawn by one torch.rand; None when nothing drops"""
-        probs = [blk.drop_prob for blk in self._layer(i)[1:]]
-        if not self.training or not any(p > 0. for p in probs):
-            return None
-        cache = self.__dict__.setdefault("_keep_cache", {})
-        key = (i, st, device)
-        ent = cache.get(key)
-        if ent is None:
-            if len(cache) >= 32:
-                cache.clear()
-            kp = torch.tensor([[1.0 - p] for p in probs], dtype=torch.float32).to(device)
-            rs = torch.arange(sum(B for B, _, _, _, _ in st), device=device).repeat_interleave(
-                torch.tensor([N for B, _, _, N, _ in st for _ in range(B)], device=device))
-            ent = cache[key] = (kp, rs)
-        kp, rs = ent
-        r = torch.rand(kp.shape[0], sum(B for B, _, _, _, _ in st), dtype=torch.float32, device=device)
-        return r.add_(kp).floor_().div_(kp).index_select(1, rs)
+    def _depths(self) -> List[int]:
+        return [cfg['n'] for cfg in self.layer_cfgs]
 
     def _run(self, imgs: List[Tensor], taps=None):
-        """-> (stream fp32 [T, C] after the last stage, pending delta, last-stage geometry); taps(i, j) selects the
-        MlpBlock outputs (stage i, block j) whose features go to taps.out (forward_return_n_last_blocks)."""
+        """-> (stream fp32 [T, C] after the last stage, pending delta, last-stage geometry); taps: see backbone.tap,
+        called after each MlpBlock with the stage's geometry."""
         cc = _CastCache()
         geo = self._geometry(imgs)
         modes = self._last_modes = self._modes(len(imgs), imgs[0].device)
         k_sc = 0
-        x, pend, prev = None, None, None
+        x, pend, prev, b = None, None, None, 0
         for i in range(self.num_layers):
             layer = self._layer(i)
             st = geo[i]
@@ -625,84 +606,43 @@ class MsViT(nn.Module):
             else:
                 x = emb.fused(ops.residual_add(x, *pend) if pend is not None else x, prev, cc)
             pend = None
-            keeps = self._stage_keeps(i, st, x.device)
+            # the DropPath scales of the AttnBlock and MlpBlock of every block, per image (the global row included)
+            scales = backbone.drop_path_scales(self, [blk.drop_prob for blk in layer[1:]],
+                                               sum(B for B, _, _, _, _ in st), x.device)
+            keeps = backbone.drop_path_rows(self, scales, [(B, N) for B, _, _, N, _ in st], x.device)
             groups = tuple((B, r0) for B, _, _, _, r0 in st)
             Ns = [N for _, _, _, N, _ in st]
             for j in range((len(layer) - 1) // 2):
                 ab, mb = layer[1 + 2 * j], layer[2 + 2 * j]
                 k1 = keeps[2 * j] if keeps is not None and ab.drop_prob > 0. else None
                 k2 = keeps[2 * j + 1] if keeps is not None and mb.drop_prob > 0. else None
-                delta, keep, dbias = pend if pend is not None else (None, None, None)
-                x, y = ops.add_layer_norm(x, delta, keep, ab.norm.weight, ab.norm.bias, ab.norm.eps, delta_bias=dbias)
                 if isinstance(ab.attn, Long2DSCSelfAttention):
-                    a = ab.attn.fused(y, groups, [(H, Wd) for _, H, Wd, _, _ in st], modes[k_sc], cc)
+                    sc_modes = modes[k_sc]
                     k_sc += 1
+                    attend = partial(ab.attn.fused, groups=groups, geo=[(H, Wd) for _, H, Wd, _, _ in st],
+                                     modes=sc_modes, cc=cc)
                 else:
-                    a = ab.attn.fused(y, groups, Ns, cc)
-                x, y = ops.add_layer_norm(x, a, k1, mb.norm.weight, mb.norm.bias, mb.norm.eps,
-                                          delta_bias=ab.attn.proj.bias)
-                pend = (mb.mlp.fused(y, cc), k2, mb.mlp.fc2.bias)
-                if taps is not None and taps(i, j):
-                    x, pend = ops.residual_add(x, *pend), None
-                    taps.out.append(self._tap_feature(i, x, st))
+                    attend = partial(ab.attn.fused, groups=groups, Ns=Ns, cc=cc)
+                x, pend = backbone.pre_norm_block(x, pend, ab.norm, attend, mb.norm, ab.attn.proj.bias,
+                                                  partial(mb.mlp.fused, cc=cc), mb.mlp.fc2.bias, k1, k2)
+                x, pend = backbone.tap(taps, b, x, pend, st)
+                b += 1
             prev = tuple((B, N, self.Nglos[i], H, Wd, r0) for B, H, Wd, N, r0 in st)
         return x, pend, geo[-1]
 
     def _tap_feature(self, i: int, x: Tensor, st) -> Tensor:
-        if i == self.num_layers - 1:  # :662-663 the final norm on the last stage's blocks
-            x = ops.LayerNormFn.apply(x, self.norm.weight, self.norm.bias, self.norm.eps, False)
-        if self.Nglos[i] > 0:  # :665-666 the global row
+        """:636-676: the global row of a block's output where the stage has one (:665-666), else its token mean"""
+        if self.Nglos[i] > 0:
             return ops.VitSplitGroupsFn.apply(x, tuple((B, H * Wd) for B, H, Wd, _, _ in st))[0]
         return ops.TokenMeanGroupsFn.apply(x, tuple((B, H, Wd, r0) for B, H, Wd, _, r0 in st))
 
-    def _features(self, imgs: List[Tensor]):
-        """-> (x_cls fp32 [sum B, C] = token mean of the final norm's tokens, x_region fp32 [sum B*N, C], geometry)"""
-        x, pend, st = self._run(imgs)
-        delta, keep, dbias = pend if pend is not None else (None, None, None)
-        _, region = ops.add_layer_norm(x, delta, keep, self.norm.weight, self.norm.bias, self.norm.eps, y_bf16=False,
-                                       delta_bias=dbias)
-        return ops.TokenMeanGroupsFn.apply(region, tuple((B, H, Wd, r0) for B, H, Wd, _, r0 in st)), region, st
-
-    def forward_features(self, x: Tensor):
-        """:581-605 -> x_cls fp32 [B, C] (and x_region fp32 [B, N, C] in dense mode)"""
-        pooled, region, st = self._features([x.float()])
-        if self.use_dense_prediction:
-            B, H, Wd, N, _ = st[0]
-            return pooled, region.view(B, N, -1)
-        return pooled
-
-    def forward_return_n_last_blocks(self, x: Tensor, n: int = 1, return_patch_avgpool: bool = False, depth=[]):
-        """:636-676: the features of the last n blocks (every MlpBlock output; stages with a global token give their
-        global row, the last stage the token mean through the final norm), concatenated"""
-        depths = [cfg['n'] for cfg in self.layer_cfgs]
-        if list(depth) != depths:
-            raise ValueError(f"depth must list the blocks per stage {depths}, got {list(depth)}")
-        if not 1 <= int(n) <= sum(depths):
-            raise ValueError(f"n must be in [1, {sum(depths)}], got {n}")
-        start = sum(depths) - int(n)
-        first = [sum(depths[:i]) for i in range(len(depths))]
-
-        def taps(i, j):
-            return first[i] + j >= start
-
-        taps.out = []
-        self._run([x.float()], taps)
-        return torch.cat(taps.out, dim=-1)
-
-    def forward(self, x):
-        """Multi-crop forward (:719-769): consecutive same-resolution crops form one group; outputs concatenated
-        group-major as the reference's per-group loop does"""
-        if not isinstance(x, list):
-            x = [x]
-        groups, start = [], 0
-        for i in range(1, len(x) + 1):
-            if i == len(x) or x[i].shape[-1] != x[start].shape[-1]:
-                groups.append((start, i))
-                start = i
-        pooled, region, st = self._features([ops.cat_adjacent(x[s:e]).float() for s, e in groups])
-        if self.use_dense_prediction:
-            return self.head(pooled), self.head_dense(region), region, [N for _, _, _, N, _ in st]
-        return self.head(pooled)
+    def _features(self, imgs: List[Tensor], taps=None):
+        """-> (x_cls fp32 [sum B, C] = token mean of the final norm's tokens, x_region fp32 [sum B*N, C], tokens per
+        image)"""
+        x, pend, st = self._run(imgs, taps)
+        region = self._final_norm(x, pend)
+        pooled = ops.TokenMeanGroupsFn.apply(region, tuple((B, H, Wd, r0) for B, H, Wd, _, r0 in st))
+        return pooled, region, [N for _, _, _, N, _ in st]
 
 
 def get_cls_model(config, is_teacher=False, use_dense_prediction=False, **kwargs):

@@ -25,8 +25,9 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import linear, ops, shadow
-from .swin_transformer import USE_GEMM2, Mlp, _CastCache, _lin_c, drop_path_keep
+from . import backbone, linear, ops, shadow
+from .backbone import MultiCropBackbone, _CastCache
+from .swin_transformer import USE_GEMM2, Mlp, _lin_c
 
 Tensor = torch.Tensor
 
@@ -147,25 +148,17 @@ class Block(nn.Module):
         self.mlp = Mlp(in_features=dim, hidden_features=int(dim * mlp_ratio), act_layer=act_layer, drop=drop)
 
     def fused_groups(self, x: Optional[Tensor], pending, grp, cc, k1: Optional[Tensor], k2: Optional[Tensor]):
-        """(x fp32 [T, C], pending = (delta bf16, keep, delta_bias) or None) -> (x, pending): the MLP branch's residual
-        add is deferred into the next fused add+LN.  k1 / k2: per-ROW DropPath scales fp32 [T] or None."""
-        delta, keep, dbias = pending if pending is not None else (None, None, None)
-        x, y = ops.add_layer_norm(x, delta, keep, self.norm1.weight, self.norm1.bias, self.norm1.eps, delta_bias=dbias)
-        a = self.attn.attend_groups(y, grp, cc)
-        x, y = ops.add_layer_norm(x, a, k1, self.norm2.weight, self.norm2.bias, self.norm2.eps,
-                                  delta_bias=self.attn.proj.bias)
-        z = self.mlp.fused(y, cc)
-        return x, (z, k2, self.mlp.fc2.bias)
+        """backbone.pre_norm_block over the sequences grp = ((B, L, row0), ...)"""
+        return backbone.pre_norm_block(x, pending, self.norm1, lambda y: self.attn.attend_groups(y, grp, cc),
+                                       self.norm2, self.attn.proj.bias, lambda y: self.mlp.fused(y, cc),
+                                       self.mlp.fc2.bias, k1, k2)
 
     def forward(self, x: Tensor, return_attention: bool = False) -> Tensor:
         """Reference signature (:110-116): x [B, N, C] -> fp32 [B, N, C]."""
         if return_attention:
             raise NotImplementedError("ViT attention maps are not implemented (forward_selfattention)")
         B, N, C = x.shape
-        k1 = k2 = None
-        if self.training and self.drop_prob > 0.:
-            k1 = drop_path_keep(B, self.drop_prob, True, x.device).repeat_interleave(N)
-            k2 = drop_path_keep(B, self.drop_prob, True, x.device).repeat_interleave(N)
+        k1, k2 = backbone.block_keeps(self, B, N, x.device)
         xs, pend = self.fused_groups(x.float().reshape(B * N, C), None, ((B, N, 0),), _CastCache(), k1, k2)
         return ops.residual_add(xs, *pend).view(B, N, C)
 
@@ -195,7 +188,7 @@ class PatchEmbed(nn.Module):
         return pe.float().view(B, -1, pe.shape[-1])
 
 
-class VisionTransformer(nn.Module):
+class VisionTransformer(MultiCropBackbone):
     """models/vision_transformer.py:142-360."""
 
     def __init__(self, img_size=[224], patch_size=16, in_chans=3, num_classes=0, embed_dim=768, depth=12,
@@ -269,101 +262,49 @@ class VisionTransformer(nn.Module):
             r0 += B * (N + 1)
         return x, tuple(grp), tg
 
-    def _keeps(self, grp, device) -> Optional[Tensor]:
-        """per-row DropPath scales fp32 [2*depth, T] (timm: floor(keep_prob + U) / keep_prob per (call, sample)), drawn
-        by one torch.rand as SwinTransformer._run does; None when no block drops."""
-        if not self.training or not any(blk.drop_prob > 0. for blk in self.blocks):
-            return None
-        cache = self.__dict__.setdefault("_kp_cache", {})
-        kp = cache.get(device)
-        if kp is None:
-            kp = cache[device] = torch.tensor([[1.0 - blk.drop_prob] for blk in self.blocks for _ in range(2)],
-                                              dtype=torch.float32).to(device)
-        rows = self.__dict__.setdefault("_rs_cache", {})
-        rs = rows.get((grp, device))
-        if rs is None:
-            if len(rows) >= 8:  # a handful of crop geometries per run; keep the cache from growing with odd batches
-                rows.clear()
-            parts, b0 = [], 0
-            for B, L, _ in grp:
-                parts.append(torch.arange(b0, b0 + B, device=device).repeat_interleave(L))
-                b0 += B
-            rs = rows[(grp, device)] = torch.cat(parts)
-        r = torch.rand(kp.shape[0], sum(g[0] for g in grp), dtype=torch.float32, device=device)
-        return r.add_(kp).floor_().div_(kp).index_select(1, rs)
+    def _depths(self) -> List[int]:
+        return [len(self.blocks)]
 
-    def _final_norm(self, x: Tensor, pend) -> Tensor:
-        delta, keep, dbias = pend if pend is not None else (None, None, None)
-        _, y = ops.add_layer_norm(x, delta, keep, self.norm.weight, self.norm.bias, self.norm.eps, y_bf16=False,
-                                  delta_bias=dbias)
-        return y
-
-    def _run(self, imgs: List[Tensor]):
-        """-> (cls fp32 [sum B, D], region fp32 [sum B*N, D], token groups)."""
+    def _run(self, imgs: List[Tensor], taps=None):
+        """-> (stream fp32 [T, D], pending delta, token groups ((B, N), ...)); taps: see backbone.tap, called with the
+        token groups."""
         cc = _CastCache()
         x, grp, tg = self._embed(imgs, cc)
-        keeps = self._keeps(grp, x.device)
+        probs = [blk.drop_prob for blk in self.blocks for _ in range(2)]
+        scales = backbone.drop_path_scales(self, probs, sum(g[0] for g in grp), x.device)
+        keeps = backbone.drop_path_rows(self, scales, [(B, L) for B, L, _ in grp], x.device)
         pend = None
         for i, blk in enumerate(self.blocks):
             k1 = k2 = None
             if keeps is not None and blk.drop_prob > 0.:
                 k1, k2 = keeps[2 * i], keeps[2 * i + 1]
             x, pend = blk.fused_groups(x, pend, grp, cc, k1, k2)
+            x, pend = backbone.tap(taps, i, x, pend, tg)
+        return x, pend, tg
+
+    def _features(self, imgs: List[Tensor], taps=None):
+        """-> (cls fp32 [sum B, D], region fp32 [sum B*N, D] = the final norm's patch tokens, patches per image)"""
+        x, pend, tg = self._run(imgs, taps)
         cls, region = ops.VitSplitGroupsFn.apply(self._final_norm(x, pend), tg)
-        return cls, region, tg
+        return cls, region, [N for _, N in tg]
 
-    def forward(self, x):
-        """Multi-crop forward (:186-231): consecutive same-resolution crops form one group; the outputs are
-        concatenated group-major exactly as the reference's per-group loop concatenates them."""
-        if not isinstance(x, list):
-            x = [x]
-        groups, start = [], 0
-        for i in range(1, len(x) + 1):
-            if i == len(x) or x[i].shape[-1] != x[start].shape[-1]:
-                groups.append((start, i))
-                start = i
-        cls, region, tg = self._run([ops.cat_adjacent(x[s:e]).float() for s, e in groups])
-        if self.use_dense_prediction:
-            return self.head(cls), self.head_dense(region), region, [N for _, N in tg]
-        return self.head(cls)
-
-    def forward_features(self, x: Tensor):
-        """:233-251 -> cls fp32 [B, D] (and the region tokens fp32 [B, N, D] in dense mode)."""
-        cls, region, tg = self._run([x.float()])
-        if self.use_dense_prediction:
-            return cls, region.view(tg[0][0], tg[0][1], -1)
-        return cls
+    def _tap_feature(self, i: int, x: Tensor, tg) -> Tensor:
+        """:339-360: the cls row of a block's normed output"""
+        return ops.VitSplitGroupsFn.apply(x, tg)[0]
 
     def forward_feature_maps(self, x: Tensor) -> Tensor:
         """:253-269 -> the final norm's output fp32 [B, 1+N, D]."""
-        cc = _CastCache()
-        xs, grp, tg = self._embed([x.float()], cc)
-        pend = None
-        for blk in self.blocks:
-            xs, pend = blk.fused_groups(xs, pend, grp, cc, None, None)
-        return self._final_norm(xs, pend).view(tg[0][0], tg[0][1] + 1, -1)
+        xs, pend, _ = self._run([x.float()])
+        return self._final_norm(xs, pend).view(x.shape[0], -1, xs.shape[-1])
 
     def forward_return_n_last_blocks(self, x: Tensor, n: int = 1, return_patch_avgpool: bool = False, depths=[]):
         """:339-360 (eval_linear.py's probe features): the final norm's cls row after each of the last n blocks,
         concatenated, plus the mean of the last block's normed patch tokens when return_patch_avgpool.  `depths` is
-        ignored, as in the reference.  A tapped block's output is materialised (residual_add) and the stream continues
-        from it."""
-        depth = len(self.blocks)
-        if not 1 <= int(n) <= depth:
-            raise ValueError(f"n must be in [1, {depth}], got {n}")
-        cc = _CastCache()
-        xs, grp, tg = self._embed([x.float()], cc)
-        out, pend, region = [], None, None
-        for i, blk in enumerate(self.blocks):
-            xs, pend = blk.fused_groups(xs, pend, grp, cc, None, None)
-            if depth - i <= int(n):
-                xs, pend = ops.residual_add(xs, *pend), None
-                y = ops.LayerNormFn.apply(xs, self.norm.weight, self.norm.bias, self.norm.eps, False)
-                cls, region = ops.VitSplitGroupsFn.apply(y, tg)
-                out.append(cls)
+        ignored, as in the reference."""
+        out, region = self._last_blocks(x, n, self._depths())
         if return_patch_avgpool:
-            B, N = tg[0]
-            out.append(ops.TokenMeanGroupsFn.apply(region, ((B, 1, N, 0),)))
+            B = x.shape[0]
+            out.append(ops.TokenMeanGroupsFn.apply(region, ((B, 1, region.shape[0] // B, 0),)))
         return torch.cat(out, dim=-1)
 
     def forward_selfattention(self, x, n=1):

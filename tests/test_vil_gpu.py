@@ -355,14 +355,20 @@ def test_step_graph_matches_eager_and_draws_fresh_modes():
     assert int(student._last_modes.abs().max()) == 0
 
 
-def test_drop_path_keeps_are_per_image_including_the_global_row():
-    from esvit_b200 import vision_longformer as V
+def test_drop_path_rows_of_a_forward_are_per_image_including_the_global_row(monkeypatch):
+    from esvit_b200 import backbone, vision_longformer as V
     m = V.msvit(drop_path_rate=0.5).cuda().train()
-    st = ((3, 56, 56, 1 + 56 * 56, 0), (2, 24, 24, 1 + 24 * 24, 3 * (1 + 56 * 56)))
-    k = m._stage_keeps(0, st, torch.device("cuda"))
+    drawn = []
+    orig = backbone.drop_path_rows
+    monkeypatch.setattr(backbone, "drop_path_rows",
+                        lambda m_, s, counts, dev: drawn.append((counts, orig(m_, s, counts, dev))) or drawn[-1][1])
+    with torch.no_grad():
+        m([torch.randn(3, 3, 224, 224, device="cuda"), torch.randn(2, 3, 96, 96, device="cuda")])
+    counts, k = drawn[0]  # stage 1
+    assert [tuple(c) for c in counts] == [(3, 1 + 56 * 56), (2, 1 + 24 * 24)]
     assert k.shape == (4, 3 * (1 + 56 * 56) + 2 * (1 + 24 * 24))
     r0 = 0
-    for B, H, W, N, _ in st:
+    for B, N in counts:
         for b in range(B):
             rows = k[:, r0:r0 + N]
             assert torch.all(rows == rows[:, :1])

@@ -347,12 +347,12 @@ def test_training_step_against_reference_fixture(G, name):
         assert_close(a, r, PATCH_W_TOL["fixture"] if k == "patch_embed.proj.weight" else TOL_BF16_GRAD, k)
 
 
-def test_drop_path_rows_match_oracle(G):
+def test_drop_path_rows_of_a_forward_match_oracle(G, monkeypatch):
     """student DropPath (linspace(0, 0.1, depth)): the per-(block, branch, image) scales the model draws, broadcast to
     the rows of every resolution group, give the oracle's forward and gradients with the same per-image scales"""
     from functools import partial
     import torch.nn as nn
-    from esvit_b200 import vision_transformer as VT
+    from esvit_b200 import backbone, vision_transformer as VT
     C = G["cases"]["p16"]
     nH = G["spec"]["num_heads"]
     m = VT.VisionTransformer(patch_size=16, mlp_ratio=4, qkv_bias=True, norm_layer=partial(nn.LayerNorm, eps=1e-6),
@@ -361,19 +361,22 @@ def test_drop_path_rows_match_oracle(G):
     m.head, m.head_dense = nn.Identity(), nn.Identity()
     m = m.cuda().train()
     drawn = []
-    orig = m._keeps
-    m._keeps = lambda grp, dev: drawn.append((grp, orig(grp, dev))) or drawn[-1][1]
+    orig = backbone.drop_path_rows
+    monkeypatch.setattr(backbone, "drop_path_rows",
+                        lambda m_, s, counts, dev: drawn.append((counts, orig(m_, s, counts, dev))) or drawn[-1][1])
     torch.manual_seed(3)
     crops = [c.cuda() for c in C["crops"]]
     cls, region, _, _ = m(crops)
-    (grp, keeps), = drawn
+    (counts, keeps), = drawn
     assert keeps is not None and float((keeps == 0).float().mean()) > 0  # something was dropped
-    okeeps = []
-    for B, L, r0 in grp:
+    okeeps, r0 = [], 0
+    for B, L in counts:
         rows = keeps[:, r0:r0 + B * L].view(keeps.shape[0], B, L)
         assert torch.equal(rows, rows[:, :, :1].expand_as(rows))  # one scale per image
         per = rows[:, :, 0].cpu().double()
         okeeps.append([(per[2 * i], per[2 * i + 1]) for i in range(len(m.blocks))])
+        r0 += B * L
+    assert r0 == keeps.shape[1]
     assert torch.equal(keeps[0], torch.ones_like(keeps[0]))  # block 0 has drop probability 0
     gen = torch.Generator().manual_seed(5)
     gc, gr = torch.randn(cls.shape, generator=gen), torch.randn(region.shape, generator=gen)
