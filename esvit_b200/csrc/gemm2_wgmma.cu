@@ -4,8 +4,10 @@
 //   D[M,N] = epi( opA(A) . opB(B) )        fp32 accumulation in registers
 //
 //   * warp specialisation: one producer warpgroup (one thread issues the TMA loads of a STAGES-deep ring of
-//     [A | B] tiles, mbarrier-synchronised) and WG = 1 or 2 consumer warpgroups, each owning 64 rows of the
-//     (64 * WG) x BN tile (wgmma m64nBNk16).  setmaxnreg moves registers from the producer to the consumers.
+//     [A | B] tiles, mbarrier-synchronised) and two consumer warpgroups (wgmma m64nBNk16); setmaxnreg moves registers
+//     from the producer to the consumers.  128-row tiles (WG = 2): cooperative, each consumer owns 64 rows of every
+//     tile.  64-row tiles (WG = 1): ping-pong, the consumers take the CTA's items alternately, the mainloops run in
+//     item order (a pair of mbarriers passes the turn), and one warpgroup's epilogue overlaps the other's mainloop.
 //   * operands K-major (nn.Linear forward: A[M,K], W[N,K]) or MN-major (a_mn / b_mn): the SAME row-major matrices
 //     read "transposed" by TMA boxes of [64 contiguous MN elements x 64 K rows] and wgmma's transpose bits, so
 //     the input-gradient GEMM dX = dY . W reads W[N,K] as it lies and the weight-gradient GEMM dW = dY^T . X reads
@@ -17,7 +19,8 @@
 //     32-byte sectors, clipped at M / N by the TMA); the multiplier comes in by TMA, issued by the producer during the
 //     mainloop.  The fp32 partials are stored from the registers.
 // Persistent: one CTA per SM, static round-robin over (split, m tile, n tile) work items; the producer runs ahead into
-// the next item's K blocks while the consumers store the previous one.
+// the next item's K blocks while the consumers store the previous one.  Neither schedule changes an element's k16
+// accumulation order: the bf16 results of every tile shape are bit-identical.
 #include <cuda.h>
 
 #include "common.cuh"
@@ -241,54 +244,65 @@ struct Params {
   int kb_per_split;   // 64-wide K blocks per split
 };
 
+// Two consumer warpgroups either way.  WG = 2 (cooperative): both work on one 128-row tile, warpgroup wg on rows
+// [64 wg, 64 wg + 64).  WG = 1 (ping-pong, PP): each warpgroup owns whole 64-row items, the CTA's items alternately, with
+// its own epilogue buffers and barriers, so one warpgroup's epilogue runs while the other's mainloop keeps the tensor
+// cores busy.
 template <int WG, int BN, int EPI>
 struct Cfg {
+  static constexpr bool PP = WG == 1;
+  static constexpr int NEP = PP ? 2 : 1;         // sets of epilogue buffers and epilogue mbarriers
   static constexpr int BM = 64 * WG;
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int BAR_BYTES = 256;
+  static constexpr int BAR_BYTES = PP ? 512 : 256;
   // bf16 epilogue staging: 64-column chunks of the tile, [BM rows][128 B] each, 128B-swizzled like a [64 x 64] TMA box
-  // (consumer warpgroup wg owns the 8 KB at wg * 8192).  EPI_BIAS: two chunk buffers; EPI_GELU: two (out, gelu') pairs;
-  // EPI_MUL: one buffer per chunk of the tile, loaded with the multiplier by TMA and overwritten in place by the result.
+  // (cooperative: consumer warpgroup wg owns the 8 KB at wg * 8192).  EPI_BIAS: two chunk buffers; EPI_GELU: two
+  // (out, gelu') pairs; EPI_MUL: one buffer per chunk of the tile, loaded with the multiplier by TMA and overwritten in
+  // place by the result.  Ping-pong: one such set per consumer warpgroup.
   static constexpr int NCHUNK = BN / 64;
   static constexpr int CHUNK_BYTES = BM * 128;
-  static constexpr int EP_BYTES = EPI == EPI_BIAS ? 2 * CHUNK_BYTES
-                                : EPI == EPI_GELU ? 4 * CHUNK_BYTES
-                                : EPI == EPI_MUL  ? NCHUNK * CHUNK_BYTES : 0;
+  static constexpr int EP_WG_BYTES = EPI == EPI_BIAS ? 2 * CHUNK_BYTES
+                                   : EPI == EPI_GELU ? 4 * CHUNK_BYTES
+                                   : EPI == EPI_MUL  ? NCHUNK * CHUNK_BYTES : 0;
+  static constexpr int EP_BYTES = NEP * EP_WG_BYTES;
   // EPI_MUL: one row of column partials per consumer warp
-  static constexpr int CS_BYTES = EPI == EPI_MUL ? 4 * WG * BN * 4 : 0;
+  static constexpr int CS_BYTES = EPI == EPI_MUL ? 8 * BN * 4 : 0;
   static constexpr int STAGES_RAW = (SMEM_LIMIT - 1024 /*alignment slack*/ - BAR_BYTES - EP_BYTES - CS_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
   static constexpr int SMEM = 1024 + STAGES * STAGE_BYTES + EP_BYTES + CS_BYTES + BAR_BYTES;
-  static constexpr int NTHREADS = 128 * (WG + 1);
-  static_assert(STAGES >= (WG == 2 && BN == 256 ? 3 : 4), "operand ring too shallow");
+  static constexpr int NTHREADS = 384;
+  // 64 x 256 multiplier items keep three 40 KB stages beside two warpgroups' 32 KB of multiplier chunks
+  static_assert(STAGES >= (BN == 256 && (WG == 2 || EPI == EPI_MUL) ? 3 : 4), "operand ring too shallow");
   static_assert(SMEM <= SMEM_LIMIT, "shared memory budget");
-  static_assert((2 * STAGES + 2 + 2 * NCHUNK) * 8 <= BAR_BYTES, "mbarrier area");
+  static_assert((2 * STAGES + 2 * NEP + 2 * NEP * NCHUNK + 2) * 8 <= BAR_BYTES, "mbarrier area");
 };
 
 // map_o: out, map_x: gelu' out (EPI_GELU) or the multiplier in (EPI_MUL); both [64 columns x 64 rows] boxes, 128B swizzle.
 // QUICK (EPI_GELU only): QuickGELU instead of the tanh GELU
 template <int WG, int BN, int EPI, int AMN, int BMN, bool QUICK = false>
-__global__ void __launch_bounds__(128 * (WG + 1), 1) gemm_kernel(const __grid_constant__ CUtensorMap map_a,
-                                                                 const __grid_constant__ CUtensorMap map_b,
-                                                                 const __grid_constant__ CUtensorMap map_o,
-                                                                 const __grid_constant__ CUtensorMap map_x,
-                                                                 const Params p) {
+__global__ void __launch_bounds__(384, 1) gemm_kernel(const __grid_constant__ CUtensorMap map_a,
+                                                      const __grid_constant__ CUtensorMap map_b,
+                                                      const __grid_constant__ CUtensorMap map_o,
+                                                      const __grid_constant__ CUtensorMap map_x,
+                                                      const Params p) {
   using C = Cfg<WG, BN, EPI>;
   constexpr int STAGES = C::STAGES, BM = C::BM, NCHUNK = C::NCHUNK;
+  constexpr bool PP = C::PP;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // [STAGES][A | B] | epilogue chunks | column partials | mbarriers; every tile and chunk 1024-byte aligned in the SHARED
-  // address space (swizzle-128B)
+  // [STAGES][A | B] | [NEP] epilogue chunks | column partials | mbarriers; every tile and chunk 1024-byte aligned in the
+  // SHARED address space (swizzle-128B)
   uint8_t* tiles = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* ep = tiles + STAGES * C::STAGE_BYTES;
-  float* cs_part = reinterpret_cast<float*>(ep + C::EP_BYTES);   // [4 WG][BN]
+  float* cs_part = reinterpret_cast<float*>(ep + C::EP_BYTES);   // [8 consumer warps][BN]
   uint64_t* full = reinterpret_cast<uint64_t*>(ep + C::EP_BYTES + C::CS_BYTES);
   uint64_t* empty = full + STAGES;
-  uint64_t* cs_full = empty + STAGES;     // EPI_MUL: every consumer warp has written its partials of a tile
-  uint64_t* cs_empty = cs_full + 1;       // ... and the fold threads have consumed them
-  uint64_t* mul_full = cs_empty + 1;      // EPI_MUL, per chunk: the multiplier has landed
-  uint64_t* mul_empty = mul_full + NCHUNK;  // ... and the TMA store of the result has read it back out
+  uint64_t* cs_full = empty + STAGES;             // [NEP] EPI_MUL: every consumer warp has written its partials of a tile
+  uint64_t* cs_empty = cs_full + C::NEP;          // ... and the fold threads have consumed them
+  uint64_t* mul_full = cs_empty + C::NEP;         // [NEP][NCHUNK] EPI_MUL, per chunk: the multiplier has landed
+  uint64_t* mul_empty = mul_full + C::NEP * NCHUNK;  // ... and the TMA store of the result has read it back out
+  uint64_t* turn = mul_empty + C::NEP * NCHUNK;   // PP, per warpgroup: the CTA's previous item has issued its mainloop
 
   const int wg = threadIdx.x >> 7;
   const int m_tiles = (p.M + BM - 1) / BM, n_tiles = (p.N + BN - 1) / BN;
@@ -298,19 +312,21 @@ __global__ void __launch_bounds__(128 * (WG + 1), 1) gemm_kernel(const __grid_co
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];\n" ::"l"(&map_a) : "memory");
     asm volatile("prefetch.tensormap [%0];\n" ::"l"(&map_b) : "memory");
+    // every count holds for both schedules: a stage, a tile's partials and a multiplier chunk are consumed by the WG
+    // warpgroups of one item
     for (int i = 0; i < STAGES; i++) { mbar_init(&full[i], 1); mbar_init(&empty[i], 128 * WG); }
-    mbar_init(cs_full, 4 * WG);
-    mbar_init(cs_empty, FOLD_THREADS);
+    for (int e = 0; e < C::NEP; e++) { mbar_init(&cs_full[e], 4 * WG); mbar_init(&cs_empty[e], FOLD_THREADS); }
     if constexpr (EPI == EPI_MUL)
-      for (int i = 0; i < NCHUNK; i++) { mbar_init(&mul_full[i], 1); mbar_init(&mul_empty[i], WG); }
+      for (int i = 0; i < C::NEP * NCHUNK; i++) { mbar_init(&mul_full[i], 1); mbar_init(&mul_empty[i], WG); }
+    if constexpr (PP) { mbar_init(&turn[0], 128); mbar_init(&turn[1], 128); }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
   __syncthreads();
 
-  if (wg == WG) {
+  if (wg == 2) {
     // ===================== TMA producer (one thread of the last warpgroup) and, for EPI_MUL, the column-sum fold =====
-    if constexpr (WG == 2) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
-    if (threadIdx.x == 128 * WG) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+    if (threadIdx.x == 256) {
       int stage = 0;
       uint32_t phase = 0;
       int local = 0;
@@ -321,14 +337,16 @@ __global__ void __launch_bounds__(128 * (WG + 1), 1) gemm_kernel(const __grid_co
         const int kb0 = split * p.kb_per_split;
         int kb1 = kb0 + p.kb_per_split; kb1 = kb1 < k_blocks ? kb1 : k_blocks;
         // EPI_MUL: multiplier chunk j of this tile, issued after K block kb0 + j so that it lands during the mainloop
-        // while the first operand stages go out ahead of it; its buffer is free once the previous tile's result chunk j
-        // has been stored
+        // while the first operand stages go out ahead of it; its buffer is free once the result chunk j of the
+        // previous tile that used the same buffer set (PP: the same warpgroup's previous item) has been stored
+        const int e = PP ? (local & 1) : 0, use = PP ? local >> 1 : local;
         auto load_mul = [&](int j) {
-          mbar_wait(&mul_empty[j], (local & 1) ^ 1);
-          const uint32_t dst = smem_u32(ep + j * C::CHUNK_BYTES);
-          mbar_expect_tx(&mul_full[j], C::CHUNK_BYTES);
+          mbar_wait(&mul_empty[e * NCHUNK + j], (use & 1) ^ 1);
+          const uint32_t dst = smem_u32(ep + e * C::EP_WG_BYTES + j * C::CHUNK_BYTES);
+          mbar_expect_tx(&mul_full[e * NCHUNK + j], C::CHUNK_BYTES);
 #pragma unroll
-          for (int h = 0; h < WG; h++) tma_load_2d(dst + h * 8192, &map_x, &mul_full[j], n0 + 64 * j, m0 + 64 * h);
+          for (int h = 0; h < WG; h++)
+            tma_load_2d(dst + h * 8192, &map_x, &mul_full[e * NCHUNK + j], n0 + 64 * j, m0 + 64 * h);
         };
         for (int kb = kb0; kb < kb1; kb++) {
           mbar_wait(&empty[stage], phase ^ 1);
@@ -354,32 +372,39 @@ __global__ void __launch_bounds__(128 * (WG + 1), 1) gemm_kernel(const __grid_co
         if constexpr (EPI == EPI_MUL)
           for (int j = kb1 - kb0; j < NCHUNK; j++) load_mul(j);
       }
-    } else if (EPI == EPI_MUL && threadIdx.x >= 128 * WG + 32 && threadIdx.x < 128 * WG + 32 + FOLD_THREADS) {
+    } else if (EPI == EPI_MUL && threadIdx.x >= 256 + 32 && threadIdx.x < 256 + 32 + FOLD_THREADS) {
       // EPI_MUL column sums: fixed-order fold of the consumer warps' partials of each tile into this CTA's private
       // workspace row, off the consumers' path.  Column c of a tile is always folded by thread c % FOLD_THREADS, whose
-      // adds to one address land in program order, and the CTA walks the same items in the same order on every run:
-      // the column sums (the fc1 bias gradient) are bit-reproducible.
-      const int t = threadIdx.x - 128 * WG - 32;
+      // adds to one address land in program order, and the CTA walks the same items in the same order on every run
+      // (PP: in item order, alternating between the two warpgroups' partial rows): the column sums (the fc1 bias
+      // gradient) are bit-reproducible.
+      const int t = threadIdx.x - 256 - 32;
       float* dst = p.colsum + (long long)blockIdx.x * p.N;
       int local = 0;
       for (int item = blockIdx.x; item < num_items; item += gridDim.x, local++) {
         const int n0 = ((item % tiles_mn) % n_tiles) * BN;
-        mbar_wait(cs_full, local & 1);
+        const int e = PP ? (local & 1) : 0, use = PP ? local >> 1 : local;
+        mbar_wait(&cs_full[e], use & 1);
         for (int c = t; c < BN && n0 + c < p.N; c += FOLD_THREADS) {
           float sum = 0.f;
 #pragma unroll
-          for (int w = 0; w < 4 * WG; w++) sum += cs_part[w * BN + c];
+          for (int w = 0; w < 4 * WG; w++) sum += cs_part[(4 * e + w) * BN + c];
           atomicAdd(dst + n0 + c, sum);
         }
-        mbar_arrive(cs_empty);
+        mbar_arrive(&cs_empty[e]);
       }
     }
   } else {
-    // ===================== consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile =====================
-    if constexpr (WG == 2) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+    // ===================== consumers: cooperative, warpgroup wg owns rows [64 wg, 64 wg + 64) of every tile; ========
+    // ===================== ping-pong, warpgroup wg owns the whole 64-row items local % 2 == wg of the CTA  ========
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
     const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
-    const int frag_row = wg * 64 + warp * 16 + (lane >> 2);   // tile row of acc[4i], acc[4i + 1]; +8 for acc[4i + 2 / 3]
+    const int row0 = PP ? 0 : 64 * wg;                        // this warpgroup's first row of the tile
+    const int frag_row = row0 + warp * 16 + (lane >> 2);      // tile row of acc[4i], acc[4i + 1]; +8 for acc[4i + 2 / 3]
     const int frag_col = 2 * (lane & 3);                      // + 8 i
+    const uint32_t rows_off = PP ? 0u : (uint32_t)wg * 8192u; // byte offset of those rows in an A tile / a chunk buffer
+    const int e = PP ? wg : 0;                                // this warpgroup's set of epilogue buffers and barriers
+    uint8_t* const my_ep = ep + e * C::EP_WG_BYTES;
     constexpr uint32_t KSTEP_A = AMN ? (2048 >> 4) : (32 >> 4), KSTEP_B = BMN ? (2048 >> 4) : (32 >> 4);
     int stage = 0;
     uint32_t phase = 0;
@@ -389,11 +414,21 @@ __global__ void __launch_bounds__(128 * (WG + 1), 1) gemm_kernel(const __grid_co
       const int m0 = (tile / n_tiles) * BM, n0 = (tile % n_tiles) * BN;
       const int kb0 = split * p.kb_per_split;
       int kb1 = kb0 + p.kb_per_split; kb1 = kb1 < k_blocks ? kb1 : k_blocks;
+      if constexpr (PP) {
+        if ((local & 1) != wg) {   // the other warpgroup's item: its K blocks pass through the ring in between
+          stage += kb1 - kb0;
+          while (stage >= STAGES) { stage -= STAGES; phase ^= 1; }
+          continue;
+        }
+        // the mainloops go in item order: wait until the previous item's wgmma have been issued
+        if (local > 0) mbar_wait(&turn[wg], ((local - 1) >> 1) & 1);
+      }
+      const int use = PP ? local >> 1 : local;   // this warpgroup's items so far: parity of its epilogue barriers
       float acc[BN / 2];
       int prev = -1;
       for (int kb = kb0; kb < kb1; kb++) {
         mbar_wait(&full[stage], phase);
-        const uint32_t sa = smem_u32(tiles + stage * C::STAGE_BYTES) + wg * 8192;   // this warpgroup's 64 rows of A
+        const uint32_t sa = smem_u32(tiles + stage * C::STAGE_BYTES) + rows_off;   // this warpgroup's 64 rows of A
         const uint64_t da = make_smem_desc(sa, AMN), db = make_smem_desc(smem_u32(tiles + stage * C::STAGE_BYTES) + C::A_BYTES, BMN);
         wgmma_fence();
 #pragma unroll
@@ -406,6 +441,7 @@ __global__ void __launch_bounds__(128 * (WG + 1), 1) gemm_kernel(const __grid_co
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
+      if constexpr (PP) mbar_arrive(&turn[wg ^ 1]);   // the other warpgroup's next mainloop may go
       wgmma_wait<0>();
       if (prev >= 0) mbar_arrive(&empty[prev]);
 
@@ -432,17 +468,17 @@ __global__ void __launch_bounds__(128 * (WG + 1), 1) gemm_kernel(const __grid_co
       // operands' out-of-bounds rows / columns were zero-filled, so those accumulators (and multipliers) are 0.
       // ldmatrix / stmatrix lane address: row (lane & 15) of the warp's 16, 16-byte column block (lane >> 4) of a pair;
       // the 128B swizzle puts 16-byte block c of row r at block c ^ (r & 7): the 8 rows of a matrix hit distinct banks.
-      if constexpr (EPI == EPI_MUL) mbar_wait(cs_empty, (local & 1) ^ 1);   // the previous tile's partials are folded
+      if constexpr (EPI == EPI_MUL) mbar_wait(&cs_empty[e], (use & 1) ^ 1);   // the previous tile's partials are folded
       const uint32_t lrow = (uint32_t)(warp * 16 + (lane & 15)) * 128u, lsw = lane & 7, lblk = lane >> 4;
       const bool leader = t == 0;   // issues this warpgroup's stores and waits for them
 #pragma unroll
       for (int c = 0; c < NCHUNK; c++) {
         uint32_t buf;   // this warpgroup's [64 rows][128 B] of the chunk buffer
         if constexpr (EPI == EPI_MUL) {
-          buf = smem_u32(ep + c * C::CHUNK_BYTES) + wg * 8192;
-          mbar_wait(&mul_full[c], local & 1);
+          buf = smem_u32(my_ep + c * C::CHUNK_BYTES) + rows_off;
+          mbar_wait(&mul_full[e * NCHUNK + c], use & 1);
         } else {
-          buf = smem_u32(ep + (c & 1) * (EPI == EPI_GELU ? 2 : 1) * C::CHUNK_BYTES) + wg * 8192;
+          buf = smem_u32(my_ep + (c & 1) * (EPI == EPI_GELU ? 2 : 1) * C::CHUNK_BYTES) + rows_off;
         }
 #pragma unroll
         for (int jj = 0; jj < 8; jj += 2) {
@@ -521,7 +557,7 @@ __global__ void __launch_bounds__(128 * (WG + 1), 1) gemm_kernel(const __grid_co
           if (leader) bulk_wait_read<0>();
         named_barrier(1 + wg, 128);
         if (leader) {
-          const int gc = n0 + 64 * c, gr = m0 + 64 * wg;
+          const int gc = n0 + 64 * c, gr = m0 + row0;
           if (gc < p.N && gr < p.M) {
             tma_store_2d(&map_o, buf, gc, gr);
             if constexpr (EPI == EPI_GELU)
@@ -530,14 +566,14 @@ __global__ void __launch_bounds__(128 * (WG + 1), 1) gemm_kernel(const __grid_co
           bulk_commit();
           if constexpr (EPI == EPI_MUL) {
             // chunk c - 1's buffer has been stored: the producer may load the next tile's multiplier into it
-            if (c > 0) { bulk_wait_read<1>(); mbar_arrive(&mul_empty[c - 1]); }
-            if (c == NCHUNK - 1) { bulk_wait_read<0>(); mbar_arrive(&mul_empty[c]); }
+            if (c > 0) { bulk_wait_read<1>(); mbar_arrive(&mul_empty[e * NCHUNK + c - 1]); }
+            if (c == NCHUNK - 1) { bulk_wait_read<0>(); mbar_arrive(&mul_empty[e * NCHUNK + c]); }
           }
         }
       }
       if constexpr (EPI == EPI_MUL) {
         __syncwarp();   // the warp's partials (lanes 0-3) are written before lane 0 releases them to the fold warps
-        if (lane == 0) mbar_arrive(cs_full);
+        if (lane == 0) mbar_arrive(&cs_full[e]);
       }
     }
     if constexpr (EPI != EPI_F32)
@@ -956,25 +992,36 @@ static int launch(const Call& c, int epi, int wg, int bn, void* stream, int* row
 
 // Tile shape policy; overridable per call through `tile` = forced_splits * 10000 + wg * 1000 + bn (0 = automatic), wg =
 // consumer warpgroups (tile rows = 64 wg).  The largest tile that still gives every SM a work item: 128 x 256 tiles read
-// the fewest operand bytes per MAC, but a GEMM with fewer tiles than SMs leaves SMs idle.
-static void pick_tile(long long M, int N, int tile, int* wg, int* bn) {
+// the fewest operand bytes per MAC, but a GEMM with fewer tiles than SMs leaves SMs idle.  fit_n (the bf16 bias / GELU
+// epilogues): no 256-wide tile where it pads N further than 128-wide ones (N = 288, 384, 576, 1152 of the Swin step),
+// whose wasted wgmma columns and half-empty last tile cost more than the extra B reads, nor at K <= 256 (4 K blocks or
+// fewer: the item is mostly epilogue, and 128-wide items overlap it better; the 65 536-wide last layers).  Measured at
+// the step's shapes, DESIGN §4.1.  The multiplier epilogue keeps 256-wide tiles: at 128 x 128 it runs slowest of the
+// four shapes.
+static bool pads_more(long long n, int wide, int narrow) {
+  return (n + wide - 1) / wide * wide > (n + narrow - 1) / narrow * narrow;
+}
+static void pick_tile(long long M, int N, int K, int tile, bool fit_n, int* wg, int* bn) {
   tile %= 10000;
   if (tile > 0) { *wg = tile / 1000; *bn = tile % 1000; return; }
   const int sms = esvit_num_sms();
+  const bool narrow = fit_n && (pads_more(N, 256, 128) || K <= 256);
   const int cand[4][2] = {{2, 256}, {2, 128}, {1, 256}, {1, 128}};
   for (const auto& cd : cand) {
-    if (cd[1] == 256 && N <= 128) continue;
+    if (cd[1] == 256 && (N <= 128 || narrow)) continue;
     const long long items = ((M + 64 * cd[0] - 1) / (64 * cd[0])) * ((N + cd[1] - 1) / cd[1]);
     if (items >= sms) { *wg = cd[0]; *bn = cd[1]; return; }
   }
   *wg = 1; *bn = 128;
 }
-// weight gradient (GEMM M = out features, N = in features, contraction over tokens): split-K supplies the parallelism
+// weight gradient (GEMM M = out features, N = in features, contraction over tokens): split-K supplies the parallelism.
+// Tiles as large as the weight allows without padding it further than the smaller shape would: 64-row (ping-pong) tiles
+// where 128-row ones pad the out features (192, 288, 576), 128-wide ones where 256-wide pad the in features (384).
 static void pick_tile_wgrad(int Nout, int Kin, int tile, int* wg, int* bn) {
   tile %= 10000;
   if (tile > 0) { *wg = tile / 1000; *bn = tile % 1000; return; }
-  *bn = Kin > 128 ? 256 : 128;
-  *wg = Nout > 64 ? 2 : 1;
+  *bn = Kin > 128 && !pads_more(Kin, 256, 128) ? 256 : 128;
+  *wg = Nout > 64 && !pads_more(Nout, 128, 64) ? 2 : 1;
 }
 
 }  // namespace hg
@@ -995,7 +1042,7 @@ ESVIT_API int esvit_gemm_bf16(const void* a, const void* b, const float* bias, v
   c.p.bias = bias; c.p.out = (bf16*)out; c.p.aux = act ? (bf16*)pre : nullptr; c.p.colsum = nullptr; c.p.part = nullptr;
   c.p.M = (int)M; c.p.N = N; c.p.K = K; c.p.splits = 1; c.p.kb_per_split = (K + hg::BK - 1) / hg::BK;
   int wg, bn;
-  hg::pick_tile(M, N, tile, &wg, &bn);
+  hg::pick_tile(M, N, K, tile, true, &wg, &bn);
   if (act == 2) return hg::launch_quick(c, wg, bn, stream);
   return hg::launch(c, act ? hg::EPI_GELU : hg::EPI_BIAS, wg, bn, stream);
 }
@@ -1012,7 +1059,7 @@ ESVIT_API int esvit_gemm_mul_colsum2(const void* a, const void* b, const void* m
   c.p.bias = nullptr; c.p.out = (bf16*)out; c.p.aux = (bf16*)mult; c.p.colsum = ws; c.p.part = nullptr;
   c.p.M = (int)M; c.p.N = N; c.p.K = K; c.p.splits = 1; c.p.kb_per_split = (K + hg::BK - 1) / hg::BK;
   int wg, bn, rows = 0;
-  hg::pick_tile(M, N, tile, &wg, &bn);
+  hg::pick_tile(M, N, K, tile, false, &wg, &bn);
   const int rc = hg::launch(c, hg::EPI_MUL, wg, bn, stream, &rows);
   if (rc != 0) return rc;
   hg::colsum_fold_kernel<<<(N + 255) / 256, 256, 0, (cudaStream_t)stream>>>(ws, rows, N, colsum);
