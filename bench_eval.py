@@ -3,6 +3,7 @@
     python bench_eval.py probe   # forward_return_n_last_blocks(x, 4, False, depths), Swin-T W7, 224^2, B = 128
     python bench_eval.py knn     # knn_classifier on synthetic ImageNet-shaped features, k in {10, 20, 100, 200}
     python bench_eval.py attn    # forward_selfattention(x, n=2), Swin-T W7, 224^2, B = 1 and 64 (analyze_models.py)
+    python bench_eval.py transforms  # the eval_linear.py / eval_knn.py input transforms on the device, B = 128 and 256
 
 probe: images/s of the CUDA path against the unmodified reference modules (oracle/_ref/, fp32, what eval_linear.py runs)
 on the same GPU and the same seeded weights, with the rel-L2 difference of their outputs.
@@ -17,6 +18,13 @@ attn: images/s of forward_selfattention(x, 2) against the unmodified reference m
 rel-L2 and max-abs difference of every map, and the probability kernel's time per image (CUDA events around every
 esvit_window_attn_probs launch) with its bytes/s against 3.35 TB/s; the bytes are the maps written plus the q/k rows read,
 computed from shapes.
+
+transforms: images/s of EvalAugment for the linear probe's training transform (LinearTrainParams: RandomResizedCrop(224)
++ flip) and the validation / k-NN transform (CenterCropParams: Resize(256, bicubic) + CenterCrop(224)) from pinned
+collated batches, host -> device copy of the sources included, on bench_augment.py's seeded mix of 500x375, 375x500,
+800x600 and 1600x1200 sources; the worker-side cost per image (JPEG decode + convert('RGB'), record, collate; one
+thread); the unmodified reference transforms' images/s per CPU core on the decoded images (oracle/_ref/, when build()
+installed it); and the Swin-T probe rate (as in `probe`) with the CPU cores the reference transforms need to feed it.
 
 Writes nothing in the tree; card name, power limit and SM clocks are read in the same run.
 """
@@ -218,9 +226,77 @@ def knn(args) -> dict:
     return res
 
 
+def transforms(args) -> dict:
+    import io
+    import numpy as np
+    from PIL import Image
+    from bench_augment import sources
+    from esvit_b200 import augment as AG
+    from oracle import eval_augment as EA
+    from oracle import reference_import as R
+    images = sources(64)
+    samplers = {"linear_train": AG.LinearTrainParams(), "center_crop": AG.CenterCropParams()}
+    aug = AG.EvalAugment()
+    res = {"mode": "transforms", "sources": "seeded mix of 500x375, 375x500, 800x600, 1600x1200", "device": {}}
+    torch.manual_seed(0)
+    for name, t in samplers.items():
+        rates = {}
+        for B in (128, 256):
+            batches = []
+            for k in range(4):
+                imgs = [images[(k * B + i) % len(images)] for i in range(B)]
+                batches.append(AG.collate_multicrop([(t(torch.from_numpy(im)), 0) for im in imgs], pin_memory=True)[0])
+            out = aug(batches[0])
+            calls = [0]
+
+            def run():
+                aug(batches[calls[0] % 4], out=out)
+                calls[0] += 1
+            s = _time(run, args.steps, args.warmup)
+            rates[B] = {"ms_per_batch": round(s * 1e3, 3), "images_per_s": round(B / s, 1),
+                        "source_mb_per_batch": round(sum(b.pixels.numel() for b in batches) / 4 / 1e6, 1)}
+        res["device"][name] = rates
+    # worker side, one thread: what stays on the DataLoader workers, against the reference transform it replaces
+    threads = torch.get_num_threads()
+    torch.set_num_threads(1)
+    n = args.host_images
+    jpegs = []
+    for im in images[:n]:
+        buf = io.BytesIO()
+        Image.fromarray(im).save(buf, "JPEG", quality=90)
+        jpegs.append(buf.getvalue())
+    worker = {}
+    for name, t in samplers.items():
+        t0 = time.perf_counter()
+        items = [(t(Image.open(io.BytesIO(j)).convert("RGB")), 0) for j in jpegs]
+        t1 = time.perf_counter()
+        AG.collate_multicrop(items)
+        t2 = time.perf_counter()
+        worker[name] = {"decode_and_record_ms": round((t1 - t0) / n * 1e3, 3), "collate_ms": round((t2 - t1) / n * 1e3, 3),
+                        "total_ms": round((t2 - t0) / n * 1e3, 3)}
+    res["worker_per_image"] = worker
+    probe_rate = probe(args)["esvit_b200"]["images_per_s"]
+    res["swin_t_probe_images_per_s"] = round(probe_rate, 1)
+    if R.available():
+        ref = EA.reference_eval_transforms(R.REF_ROOT)
+        pils = [Image.open(io.BytesIO(j)).convert("RGB") for j in jpegs]
+        per_core = {}
+        for name, key in (("linear_train", "train_transform"), ("center_crop", "val_transform")):
+            ref[key](pils[0])
+            t0 = time.perf_counter()
+            for p in pils:
+                ref[key](p)
+            s = (time.perf_counter() - t0) / n
+            per_core[name] = {"ms_per_image": round(s * 1e3, 3), "images_per_s": round(1 / s, 1),
+                              "cores_to_feed_swin_t_probe": round(probe_rate * s, 1)}
+        res["reference_per_core"] = per_core
+    torch.set_num_threads(threads)
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("mode", choices=["probe", "knn", "attn"])
+    ap.add_argument("mode", choices=["probe", "knn", "attn", "transforms"])
     ap.add_argument("--batch", type=int, default=128)
     ap.add_argument("--batches", default="1,64", help="attn: batch sizes")
     ap.add_argument("--steps", type=int, default=10)
@@ -234,12 +310,13 @@ def main():
     ap.add_argument("--temperature", type=float, default=0.07)
     ap.add_argument("--noise", type=float, default=5.0)
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--host-images", type=int, default=40, help="transforms: images the worker-side timings run over")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("bench_eval.py needs a CUDA device")
     torch.backends.cuda.matmul.allow_tf32 = False  # the reference arms run fp32
     before = card()
-    res = {"probe": probe, "knn": knn, "attn": attn}[args.mode](args)
+    res = {"probe": probe, "knn": knn, "attn": attn, "transforms": transforms}[args.mode](args)
     res["card"] = before
     res["card_after"] = card()
     print(json.dumps(res))

@@ -94,6 +94,9 @@ SIGNATURES = {
     "esvit_augment_coeffs": [P, P, P, I, I, P],
     "esvit_augment_resize_h": [P, P, P, P, P, I, L, P],
     "esvit_augment_color": [P, P, P, P, P, I, I, I, P],
+    "esvit_augment_eval_coeffs": [P, P, P, I, I, P],
+    "esvit_augment_eval_resize_h": [P, P, P, P, P, I, I, L, P],
+    "esvit_augment_eval_resize_v": [P, P, P, P, P, I, I, P],
 }
 
 _lib = None

@@ -14,6 +14,13 @@
 //                    the sampled order (uint8 after each, as Pillow), grayscale, the 3+3 box-blur passes of Pillow's
 //                    GaussianBlur, solarize, and ToTensor + Normalize in fp32 with streaming stores.
 //
+// The evaluation transforms (eval_linear.py / eval_knn.py: RandomResizedCrop(bilinear) + flip, Resize(256, bicubic) +
+// CenterCrop) are one geometry per image: crop a box, resize it to (rh, rw), keep the S x S output window at (oy, ox),
+// optionally flip.  Their kernels share the coefficient and horizontal-pass code above:
+//   eval_coeffs_kernel    the window's tables of both axes, bilinear or bicubic per image;
+//   eval_resize_h_kernel  the horizontal pass over the box rows the window's vertical taps touch;
+//   eval_resize_v_kernel  the vertical pass, ToTensor + Normalize, coalesced fp32 stores of [B, 3, S, S].
+//
 // Every float/double expression that Pillow evaluates as a multiply followed by an add is written with _rn intrinsics
 // so that no FMA contraction changes its rounding.
 #include "common.cuh"
@@ -29,40 +36,55 @@ enum { M_SRC, M_H, M_W, M_S, M_TMP, M_COEF, M_KH, M_KV, M_OUT, NMETA };
 
 constexpr int PREC = 22;  // Pillow's PRECISION_BITS for 8-bit images
 
-static __device__ __forceinline__ double bicubic(double x) {  // Pillow's bicubic_filter, a = -0.5
-  const double a = -0.5;
-  if (x < 0.0) x = -x;
-  if (x < 1.0) return __dadd_rn(__dmul_rn(__dmul_rn(__dsub_rn(__dmul_rn(a + 2.0, x), a + 3.0), x), x), 1.0);
-  if (x < 2.0) return __dmul_rn(__dsub_rn(__dmul_rn(__dadd_rn(__dmul_rn(__dsub_rn(x, 5.0), x), 8.0), x), 4.0), a);
-  return 0.0;
-}
+struct Bicubic {  // Pillow's bicubic_filter, a = -0.5
+  static constexpr double support = 2.0;
+  static __device__ __forceinline__ double filter(double x) {
+    const double a = -0.5;
+    if (x < 0.0) x = -x;
+    if (x < 1.0) return __dadd_rn(__dmul_rn(__dmul_rn(__dsub_rn(__dmul_rn(a + 2.0, x), a + 3.0), x), x), 1.0);
+    if (x < 2.0) return __dmul_rn(__dsub_rn(__dmul_rn(__dadd_rn(__dmul_rn(__dsub_rn(x, 5.0), x), 8.0), x), 4.0), a);
+    return 0.0;
+  }
+};
 
-// Table of one axis at tab: bounds [S][2] (first input index, tap count), then coefficients [S][ksize].
-static __device__ void axis_coeffs(int in_size, int S, int ksize, int o, int* tab) {
-  const double scale = (double)in_size / S;
+struct Bilinear {  // Pillow's bilinear_filter
+  static constexpr double support = 1.0;
+  static __device__ __forceinline__ double filter(double x) {
+    if (x < 0.0) x = -x;
+    return x < 1.0 ? __dsub_rn(1.0, x) : 0.0;
+  }
+};
+
+// Entry i of the table of one axis of a resize in_size -> out_size whose outputs [o0, o0 + n) are kept, at tab:
+// bounds [n][2] (first input index, tap count), then coefficients [n][ksize].  Pillow computes every output from its own
+// taps, so a window's entries are those of the whole resize.
+template <class Filter>
+static __device__ void axis_coeffs(int in_size, int out_size, int o0, int n, int ksize, int i, int* tab) {
+  const double scale = (double)in_size / out_size;
   const double filterscale = scale < 1.0 ? 1.0 : scale;
-  const double support = __dmul_rn(2.0, filterscale);
-  const double center = __dmul_rn(o + 0.5, scale);
+  const double support = __dmul_rn(Filter::support, filterscale);
+  const double center = __dmul_rn((o0 + i) + 0.5, scale);
   const double ss = 1.0 / filterscale;
   int xmin = (int)__dadd_rn(__dsub_rn(center, support), 0.5);
   if (xmin < 0) xmin = 0;
   int xmax = (int)__dadd_rn(__dadd_rn(center, support), 0.5);
   if (xmax > in_size) xmax = in_size;
   xmax -= xmin;
-  int* k = tab + 2 * S + (long long)o * ksize;
+  int* k = tab + 2 * n + (long long)i * ksize;
   double ww = 0.0;
-  for (int x = 0; x < xmax; x++) ww = __dadd_rn(ww, bicubic(__dmul_rn(__dadd_rn(__dsub_rn((double)(x + xmin), center), 0.5), ss)));
+  for (int x = 0; x < xmax; x++)
+    ww = __dadd_rn(ww, Filter::filter(__dmul_rn(__dadd_rn(__dsub_rn((double)(x + xmin), center), 0.5), ss)));
   for (int x = 0; x < ksize; x++) {
     double w = 0.0;
     if (x < xmax) {
-      w = bicubic(__dmul_rn(__dadd_rn(__dsub_rn((double)(x + xmin), center), 0.5), ss));
+      w = Filter::filter(__dmul_rn(__dadd_rn(__dsub_rn((double)(x + xmin), center), 0.5), ss));
       if (ww != 0.0) w = __ddiv_rn(w, ww);
     }
     const double f = __dmul_rn(w, (double)(1 << PREC));
     k[x] = w < 0 ? (int)__dadd_rn(-0.5, f) : (int)__dadd_rn(0.5, f);
   }
-  tab[2 * o] = xmin;
-  tab[2 * o + 1] = xmax;
+  tab[2 * i] = xmin;
+  tab[2 * i + 1] = xmax;
 }
 
 // grid (ceil(maxS / 128), 2, ncrops): one thread per (crop, axis, output index)
@@ -74,8 +96,8 @@ __global__ void __launch_bounds__(128) coeffs_kernel(const double* __restrict__ 
   if (o >= S) return;
   const int kh = (int)m[M_KH], kv = (int)m[M_KV];
   int* tab = coef + m[M_COEF];
-  if (blockIdx.y == 0) axis_coeffs((int)p[P_W], S, kh, o, tab);
-  else axis_coeffs((int)p[P_H], S, kv, o, tab + (long long)S * (2 + kh));
+  if (blockIdx.y == 0) axis_coeffs<Bicubic>((int)p[P_W], S, 0, S, kh, o, tab);
+  else axis_coeffs<Bicubic>((int)p[P_H], S, 0, S, kv, o, tab + (long long)S * (2 + kh));
 }
 
 static __device__ __forceinline__ uint8_t clip8(int ss) {  // Pillow's clip8 of a PRECISION_BITS accumulator
@@ -83,18 +105,11 @@ static __device__ __forceinline__ uint8_t clip8(int ss) {  // Pillow's clip8 of 
   return (uint8_t)(v < 0 ? 0 : v > 255 ? 255 : v);
 }
 
-// grid (G, ncrops): tmp[y][flip ? S-1-ox : ox][c] = horizontal pass of box row y, for every row of the box
-__global__ void __launch_bounds__(256) resize_h_kernel(const uint8_t* __restrict__ src, const double* __restrict__ params,
-                                                       const long long* __restrict__ meta, const int* __restrict__ coef,
-                                                       uint8_t* __restrict__ tmp) {
-  const long long* m = meta + (long long)blockIdx.y * NMETA;
-  const double* p = params + (long long)blockIdx.y * NPARAM;
-  const int S = (int)m[M_S], W = (int)m[M_W], kh = (int)m[M_KH];
-  const int top = (int)p[P_TOP], left = (int)p[P_LEFT], h = (int)p[P_H], flip = p[P_FLIP] != 0.0;
-  const int* tab = coef + m[M_COEF];
-  const uint8_t* img = src + m[M_SRC];
-  uint8_t* out = tmp + m[M_TMP];
-  const long long n = (long long)h * S;
+// out[y][flip ? S-1-ox : ox][c] = horizontal pass of source row top + y, for y in [0, rows); grid-stride over blockIdx.x
+static __device__ __forceinline__ void resize_h_rows(const uint8_t* __restrict__ img, int W, int top, int left, int rows,
+                                                     int S, const int* __restrict__ tab, int kh, bool flip,
+                                                     uint8_t* __restrict__ out) {
+  const long long n = (long long)rows * S;
   for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) {
     const int y = (int)(e / S), ox = (int)(e - (long long)y * S);
     const int xmin = tab[2 * ox], xn = tab[2 * ox + 1];
@@ -112,6 +127,37 @@ __global__ void __launch_bounds__(256) resize_h_kernel(const uint8_t* __restrict
     o[1] = clip8(s1);
     o[2] = clip8(s2);
   }
+}
+
+// grid (G, ncrops): tmp[y][flip ? S-1-ox : ox][c] = horizontal pass of box row y, for every row of the box
+__global__ void __launch_bounds__(256) resize_h_kernel(const uint8_t* __restrict__ src, const double* __restrict__ params,
+                                                       const long long* __restrict__ meta, const int* __restrict__ coef,
+                                                       uint8_t* __restrict__ tmp) {
+  const long long* m = meta + (long long)blockIdx.y * NMETA;
+  const double* p = params + (long long)blockIdx.y * NPARAM;
+  resize_h_rows(src + m[M_SRC], (int)m[M_W], (int)p[P_TOP], (int)p[P_LEFT], (int)p[P_H], (int)m[M_S],
+                coef + m[M_COEF], (int)m[M_KH], p[P_FLIP] != 0.0, tmp + m[M_TMP]);
+}
+
+// ToTensor (u / 255) then Normalize ((x - mean) / std) in fp32, IEEE divisions in torchvision's order
+static __device__ __forceinline__ float to_tensor_normalize(int u, float mu, float sd) {
+  return __fdiv_rn(__fsub_rn(__fdiv_rn((float)u, 255.f), mu), sd);
+}
+
+// vertical pass of one output pixel: taps k[0, yn) down a column of a uint8 [rows, S, 3] intermediate, from col
+static __device__ __forceinline__ void resize_v_px(const uint8_t* __restrict__ col, int S, const int* __restrict__ k,
+                                                   int yn, uint8_t& r, uint8_t& g, uint8_t& b) {
+  int s0 = 1 << (PREC - 1), s1 = s0, s2 = s0;
+  for (int y = 0; y < yn; y++) {
+    const int w = k[y];
+    const uint8_t* px = col + (long long)y * S * 3;
+    s0 += px[0] * w;
+    s1 += px[1] * w;
+    s2 += px[2] * w;
+  }
+  r = clip8(s0);
+  g = clip8(s1);
+  b = clip8(s2);
 }
 
 // Image.blend(a, b, f) on 8-bit bands: a + f * (b - a) in fp32, truncated, clipped
@@ -216,20 +262,9 @@ __global__ void __launch_bounds__(1024, 1) color_kernel(const double* __restrict
   const uint8_t* t8 = tmp + m[M_TMP];
   for (int q = threadIdx.x; q < n; q += blockDim.x) {
     const int oy = q / S, ox = q - oy * S;
-    const int ymin = tab[2 * oy], yn = tab[2 * oy + 1];
-    const int* k = tab + 2 * S + (long long)oy * kv;
-    const uint8_t* col = t8 + ((long long)ymin * S + ox) * 3;
-    int s0 = 1 << (PREC - 1), s1 = s0, s2 = s0;
-    for (int y = 0; y < yn; y++) {
-      const int w = k[y];
-      const uint8_t* px = col + (long long)y * S * 3;
-      s0 += px[0] * w;
-      s1 += px[1] * w;
-      s2 += px[2] * w;
-    }
-    R[q] = clip8(s0);
-    G[q] = clip8(s1);
-    B[q] = clip8(s2);
+    const int ymin = tab[2 * oy];
+    resize_v_px(t8 + ((long long)ymin * S + ox) * 3, S, tab + 2 * S + (long long)oy * kv, tab[2 * oy + 1], R[q], G[q],
+                B[q]);
   }
   __syncthreads();
 
@@ -291,7 +326,7 @@ __global__ void __launch_bounds__(1024, 1) color_kernel(const double* __restrict
       }
     }
   }
-  // solarize, ToTensor (u / 255), Normalize ((x - mean) / std): fp32, streaming stores of [3, S, S]
+  // solarize, ToTensor + Normalize: fp32, streaming stores of [3, S, S]
   const bool solar = p[P_SOLAR] != 0.0;
   float* out = reinterpret_cast<float*>(m[M_OUT]);
   for (int ch = 0; ch < 3; ch++) {
@@ -300,9 +335,72 @@ __global__ void __launch_bounds__(1024, 1) color_kernel(const double* __restrict
     for (int q = threadIdx.x; q < n; q += blockDim.x) {
       int u = P[q];
       if (solar && u >= 128) u = 255 - u;
-      __stcs(out + (long long)ch * n + q, __fdiv_rn(__fsub_rn(__fdiv_rn((float)u, 255.f), mu), sd));
+      __stcs(out + (long long)ch * n + q, to_tensor_normalize(u, mu, sd));
     }
   }
+}
+
+// ---- evaluation transforms -------------------------------------------------------------------------------------------
+// float64 record of one image (esvit_b200/augment.py EVAL_FIELDS): crop box, resized size, output window, flip, Pillow
+// resample code (2 bilinear, 3 bicubic)
+enum { R_TOP, R_LEFT, R_H, R_W, R_RH, R_RW, R_OY, R_OX, R_SIZE, R_FLIP, R_INTERP, NREC };
+// int64 per-image geometry (esvit_b200/augment.py): source byte offset, source W, first box row of the window's vertical
+// taps and their row count, intermediate byte offset, coefficient-table offset (int32 elements), horizontal / vertical
+// tap counts
+enum { E_SRC, E_W, E_Y0, E_ROWS, E_TMP, E_COEF, E_KH, E_KV, NEMETA };
+constexpr int PIL_BICUBIC = 3;
+
+template <class Filter>
+static __device__ void eval_axis(const double* r, int axis, int S, int kh, int kv, int i, int* tab) {
+  if (axis == 0) axis_coeffs<Filter>((int)r[R_W], (int)r[R_RW], (int)r[R_OX], S, kh, i, tab);
+  else axis_coeffs<Filter>((int)r[R_H], (int)r[R_RH], (int)r[R_OY], S, kv, i, tab + (long long)S * (2 + kh));
+}
+
+// grid (ceil(S / 128), 2, nimg): one thread per (image, axis, window output)
+__global__ void __launch_bounds__(128) eval_coeffs_kernel(const double* __restrict__ rec,
+                                                          const long long* __restrict__ meta, int* __restrict__ coef,
+                                                          int S) {
+  const long long* m = meta + (long long)blockIdx.z * NEMETA;
+  const double* r = rec + (long long)blockIdx.z * NREC;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= S) return;
+  const int kh = (int)m[E_KH], kv = (int)m[E_KV];
+  int* tab = coef + m[E_COEF];
+  if (r[R_INTERP] == PIL_BICUBIC) eval_axis<Bicubic>(r, blockIdx.y, S, kh, kv, i, tab);
+  else eval_axis<Bilinear>(r, blockIdx.y, S, kh, kv, i, tab);
+}
+
+// grid (G, nimg): tmp[y][flip ? S-1-ox : ox][c] for box rows y0 + y, y in [0, rows)
+__global__ void __launch_bounds__(256) eval_resize_h_kernel(const uint8_t* __restrict__ src,
+                                                            const double* __restrict__ rec,
+                                                            const long long* __restrict__ meta,
+                                                            const int* __restrict__ coef, uint8_t* __restrict__ tmp,
+                                                            int S) {
+  const long long* m = meta + (long long)blockIdx.y * NEMETA;
+  const double* r = rec + (long long)blockIdx.y * NREC;
+  resize_h_rows(src + m[E_SRC], (int)m[E_W], (int)r[R_TOP] + (int)m[E_Y0], (int)r[R_LEFT], (int)m[E_ROWS], S,
+                coef + m[E_COEF], (int)m[E_KH], r[R_FLIP] != 0.0, tmp + m[E_TMP]);
+}
+
+// grid (ceil(S^2 / 256), nimg): one thread per output pixel, consecutive threads on consecutive columns, so each
+// channel plane of out [nimg, 3, S, S] is written with coalesced stores
+__global__ void __launch_bounds__(256) eval_resize_v_kernel(const long long* __restrict__ meta,
+                                                            const int* __restrict__ coef,
+                                                            const uint8_t* __restrict__ tmp,
+                                                            const float* __restrict__ norm, float* __restrict__ out,
+                                                            int S) {
+  const long long* m = meta + (long long)blockIdx.y * NEMETA;
+  const int n = S * S, q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= n) return;
+  const int oy = q / S, ox = q - oy * S;
+  const int* tab = coef + m[E_COEF] + (long long)S * (2 + (int)m[E_KH]);
+  const int ymin = tab[2 * oy] - (int)m[E_Y0];
+  uint8_t u[3];
+  resize_v_px(tmp + m[E_TMP] + ((long long)ymin * S + ox) * 3, S, tab + 2 * S + (long long)oy * (int)m[E_KV],
+              tab[2 * oy + 1], u[0], u[1], u[2]);
+  float* o = out + (long long)blockIdx.y * 3 * n + q;
+#pragma unroll
+  for (int ch = 0; ch < 3; ch++) __stcs(o + (long long)ch * n, to_tensor_normalize(u[ch], norm[ch], norm[3 + ch]));
 }
 
 }  // namespace aug
@@ -332,5 +430,29 @@ ESVIT_API int esvit_augment_color(const double* params, const long long* meta, c
   cudaError_t e = cudaFuncSetAttribute(color_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e != cudaSuccess) return (int)e;
   color_kernel<<<ncrops, 1024, smem, (cudaStream_t)stream>>>(params, meta, coef, tmp, norm, crop0);
+  ESVIT_LAUNCH_CHECK();
+}
+
+ESVIT_API int esvit_augment_eval_coeffs(const double* rec, const long long* meta, int* coef, int nimg, int S,
+                                        void* stream) {
+  if (nimg <= 0 || nimg > 65535 || S <= 0) return ESVIT_ERR_BAD_ARG;
+  eval_coeffs_kernel<<<dim3((S + 127) / 128, 2, nimg), 128, 0, (cudaStream_t)stream>>>(rec, meta, coef, S);
+  ESVIT_LAUNCH_CHECK();
+}
+
+ESVIT_API int esvit_augment_eval_resize_h(const uint8_t* src, const double* rec, const long long* meta, const int* coef,
+                                          uint8_t* tmp, int nimg, int S, long long max_pixels, void* stream) {
+  if (nimg <= 0 || nimg > 65535 || S <= 0 || max_pixels <= 0) return ESVIT_ERR_BAD_ARG;
+  const long long blocks = (max_pixels + 255) / 256;
+  const int gx = (int)(blocks < 64 ? blocks : 64);
+  eval_resize_h_kernel<<<dim3(gx, nimg), 256, 0, (cudaStream_t)stream>>>(src, rec, meta, coef, tmp, S);
+  ESVIT_LAUNCH_CHECK();
+}
+
+ESVIT_API int esvit_augment_eval_resize_v(const long long* meta, const int* coef, const uint8_t* tmp, const float* norm,
+                                          float* out, int nimg, int S, void* stream) {
+  if (nimg <= 0 || nimg > 65535 || S <= 0 || (long long)S * S > 0x7fffffffLL) return ESVIT_ERR_BAD_ARG;
+  const int gx = (int)(((long long)S * S + 255) / 256);
+  eval_resize_v_kernel<<<dim3(gx, nimg), 256, 0, (cudaStream_t)stream>>>(meta, coef, tmp, norm, out, S);
   ESVIT_LAUNCH_CHECK();
 }

@@ -346,6 +346,25 @@ int esvit_augment_resize_h(const unsigned char* src, const double* params, const
 int esvit_augment_color(const double* params, const long long* meta, const int* coef, const unsigned char* tmp,
                         const float* norm, int crop0, int ncrops, int S, void* stream);
 
+/* ---- evaluation transforms on decoded uint8 images ---------------------------- eval_linear.py:50-61, eval_knn.py:48-53
+ * RandomResizedCrop(224, bilinear) + RandomHorizontalFlip, or Resize(256, bicubic) + CenterCrop(224), then ToTensor +
+ * Normalize, with Pillow's arithmetic, for one crop per image (esvit_b200/augment.py EvalAugment builds the arguments).
+ * Each image's crop box is resized to (rh, rw) and only the S x S output window at (oy, ox) is computed.
+ * rec fp64 [nimg, 11] (augment.EVAL_FIELDS: box top, left, h, w, rh, rw, oy, ox, S, flip, Pillow resample code 2 / 3);
+ * meta int64 [nimg, 8]: source byte offset into src (uint8 HWC), source W, first box row y0 the window's vertical taps
+ * read and their row count, byte offset into tmp (uint8 [rows, S, 3] per image), int32 offset into coef
+ * (S * (4 + kh + kv) per image), horizontal / vertical tap counts kh = 2 ceil(support * max(1, w / rw)) + 1 and kv
+ * (same with h / rh), support 1 (bilinear) or 2 (bicubic).
+ * eval_coeffs: both axes' window bounds and 22-bit fixed-point coefficients into coef.
+ * eval_resize_h: the horizontal pass (flip applied) of box rows [y0, y0 + rows) into tmp; max_pixels = max rows * S.
+ * eval_resize_v: the vertical pass, ToTensor + Normalize with norm fp32 [6] = (mean[3], std[3]) into out fp32
+ *   [nimg, 3, S, S], S^2 < 2^31. */
+int esvit_augment_eval_coeffs(const double* rec, const long long* meta, int* coef, int nimg, int S, void* stream);
+int esvit_augment_eval_resize_h(const unsigned char* src, const double* rec, const long long* meta, const int* coef,
+                                unsigned char* tmp, int nimg, int S, long long max_pixels, void* stream);
+int esvit_augment_eval_resize_v(const long long* meta, const int* coef, const unsigned char* tmp, const float* norm,
+                                float* out, int nimg, int S, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
