@@ -54,6 +54,8 @@ SIGNATURES = {
     "esvit_row_softmax_q": [P, P, F, P, P, L, I, P],
     "esvit_dino_ce_q_fwd": [P, P, P, P, P, F, P, L, I, P],
     "esvit_dino_ce_q_bwd": [P, P, P, P, P, P, P, F, P, L, I, P],
+    "esvit_mixup_q_kpad": [I],
+    "esvit_mixup_q": [P, P, I, I, I, F, P, P, P, P],
     "esvit_colsum_workspace_rows": [],
     "esvit_colsum": [P, L, I, P, P, P],
     "esvit_center_ema": [P, P, F, F, P, I, P],
@@ -145,7 +147,8 @@ def call(name: str, *args) -> None:
 
 # ---- instrumentation used by bench.py (launch counting; live CUDA-event timing of one entry point) --------------
 # kernels launched per call of each entry point (entries that launch more than one kernel are computed per call)
-_LAUNCHES = {"esvit_colsum": 2, "esvit_gemm_mul_colsum": 2, "esvit_gemm_mul_colsum2": 2, "esvit_gemm_wgrad": 2}  # GEMM + fold
+_LAUNCHES = {"esvit_colsum": 2, "esvit_gemm_mul_colsum": 2, "esvit_gemm_mul_colsum2": 2, "esvit_gemm_wgrad": 2,
+             "esvit_mixup_q": 2}  # GEMM + fold; mixup weights + product
 _launch_count = 0
 _timed_names = set()
 _timed_events = []
@@ -169,6 +172,7 @@ _META = {
     "esvit_dino_ce_q_fwd": lambda a: {"rows": int(a[-3]), "K": int(a[-2])},
     "esvit_dino_ce_q_bwd": lambda a: {"rows": int(a[-3]), "K": int(a[-2])},
     "esvit_row_softmax_q": lambda a: {"rows": int(a[-3]), "K": int(a[-2])},
+    "esvit_mixup_q": lambda a: {"ncrops": int(a[2]), "B": int(a[3]), "K": int(a[4])},
     "esvit_conv_im2col": lambda a: {"B": int(a[3]), "C": int(a[4]), "H": int(a[5]), "W": int(a[6]), "k": int(a[7]),
                                     "s": int(a[8]), "p": int(a[9]), "Kp": int(a[10])},
     "esvit_conv_col2im": lambda a: {"B": int(a[2]), "C": int(a[3]), "H": int(a[4]), "W": int(a[5]), "k": int(a[6]),

@@ -509,6 +509,150 @@ __global__ void __launch_bounds__(LT) dino_ce_q_bwd_kernel(
   }
 }
 
+// ---- mixup targets (main_esvit.py:638-641): one mixed teacher row per student row -----------------------------------
+// Student row r = (v, b) of the mixup loss pairs with q~_r = sum_{iq != v} sum_j T_v[j, b] q^{iq}_j, of mass
+// C_r = sum_{iq != v} sum_j T_v[j, b].  For non-negative T, q^_r = q~_r / C_r is a probability row, stored in the q12 format
+// above, and the loss is the CE of q^ at n_r = 1 and weight w_r = C_r / (n_terms * B) (DESIGN.md §4.8).
+//   mixup_weights_kernel: one warp per student row: C_r, w_r and the row of Wn[r, i] = W[(iq, j), r] / C_r (i = iq*B + j,
+//     zero-padded to Kp), scaled by 2^14 and split into fp16 hi + lo parts, so the tensor-core product carries ~22 bits of
+//     every weight.  (Unscaled, weights below 2^-14 are fp16 subnormals: a weight of 1e-5 met by a teacher probability
+//     near 1 lost 3e-3 of the product.)
+//   mixup_q_kernel: q^[R, K] = Wn[R, Kp] . q12[Kp, K] * 2^-14 with mma.sync m16n8k16 (fp16 in, fp32 accumulate), hi and lo.
+constexpr float MX_WSCALE = 16384.f;  // Wn <= 1 -> <= 2^14: hi normal down to Wn = 2^-28, lo down to Wn = 2^-17
+__global__ void __launch_bounds__(256) mixup_weights_kernel(const float* __restrict__ T, int ncrops, int B, int Kp,
+                                                            float w_scale, __half* __restrict__ a_hi,
+                                                            __half* __restrict__ a_lo, float* __restrict__ w) {
+  const int lane = threadIdx.x & 31;
+  const long long r = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (r >= (long long)ncrops * B) return;
+  const int v = (int)(r / B), b = (int)(r % B);
+  const float* Tv = T + (long long)v * B * B;  // T_v[j, b] at Tv[j * B + b]
+  float c = 0.f;
+  for (int j = lane; j < B; j += 32) c += Tv[(long long)j * B + b];
+  c = warp_sum(c);
+  const float C = v < 2 ? c : 2.f * c;  // global views pair with the other global view only
+  if (lane == 0) w[r] = C * w_scale;
+  for (int i = lane; i < Kp; i += 32) {
+    const int iq = i / B, j = i - iq * B;
+    const float x = (i < 2 * B && iq != v && C > 0.f) ? __fdiv_rn(Tv[(long long)j * B + b], C) * MX_WSCALE : 0.f;
+    const __half h = __float2half_rn(x);
+    a_hi[r * Kp + i] = h;
+    a_lo[r * Kp + i] = __float2half_rn(x - __half2float(h));
+  }
+}
+
+constexpr int MX_BM = 128, MX_BN = 128, MX_KC = 32, MX_T = 256;
+constexpr int MX_AS = MX_KC + 8, MX_QS = MX_BN + 8;  // padded smem rows (halves): conflict-free ldmatrix / epilogue
+struct MixSmem {
+  union {
+    struct {
+      __half a_hi[MX_BM][MX_AS], a_lo[MX_BM][MX_AS];
+      __half q[MX_KC][MX_QS];
+    } ld;
+    __half out[MX_BM][MX_QS];
+  };
+};
+
+__device__ __forceinline__ void ldsm_x4(uint32_t* r, const void* p, bool trans) {
+  const unsigned a = (unsigned)__cvta_generic_to_shared(p);
+  if (trans)
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];\n"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(a));
+  else
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(a));
+}
+
+__device__ __forceinline__ void mma_f16(float* d, const uint32_t* a, const uint32_t* b) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
+               "{%0,%1,%2,%3};\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
+
+// CTA: 128 student rows x 128 columns; 8 warps as 2 (rows) x 4 (columns), 64 x 32 each.  The teacher block (2B x K fp16,
+// 16.8 MB at B = 64) is re-read from L2 by each of the R / 128 row tiles; the R x K fp16 output is the HBM traffic.
+__global__ void __launch_bounds__(MX_T) mixup_q_kernel(const __half* __restrict__ a_hi, const __half* __restrict__ a_lo,
+                                                       const __half* __restrict__ q, __half* __restrict__ out, int R,
+                                                       int Rt, int K, int Kp) {
+  __shared__ __align__(16) MixSmem sm;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wm = warp >> 2, wn = warp & 3;
+  const int n0 = blockIdx.x * MX_BN;
+  const long long m0 = (long long)blockIdx.y * MX_BM;
+  float acc[4][4][4];
+#pragma unroll
+  for (int mt = 0; mt < 4; mt++)
+#pragma unroll
+    for (int nt = 0; nt < 4; nt++)
+#pragma unroll
+      for (int e = 0; e < 4; e++) acc[mt][nt][e] = 0.f;
+
+  for (int k0 = 0; k0 < Kp; k0 += MX_KC) {
+#pragma unroll
+    for (int u = 0; u < 2; u++) {  // weights: 128 rows x 32 halves, hi and lo
+      const int idx = tid + u * MX_T, row = idx >> 2, c8 = (idx & 3) * 8;
+      const long long gr = m0 + row;
+      uint4 vh = make_uint4(0, 0, 0, 0), vl = vh;
+      if (gr < R) {
+        vh = *reinterpret_cast<const uint4*>(a_hi + gr * Kp + k0 + c8);
+        vl = *reinterpret_cast<const uint4*>(a_lo + gr * Kp + k0 + c8);
+      }
+      *reinterpret_cast<uint4*>(&sm.ld.a_hi[row][c8]) = vh;
+      *reinterpret_cast<uint4*>(&sm.ld.a_lo[row][c8]) = vl;
+    }
+#pragma unroll
+    for (int u = 0; u < 2; u++) {  // teacher probabilities: 32 rows x 128 columns (zero past the last row / column)
+      const int idx = tid + u * MX_T, row = idx >> 4, c8 = (idx & 15) * 8;
+      const int gi = k0 + row, gk = n0 + c8;
+      uint4 vq = make_uint4(0, 0, 0, 0);
+      if (gi < Rt && gk < K) vq = *reinterpret_cast<const uint4*>(q + (long long)gi * K + gk);
+      *reinterpret_cast<uint4*>(&sm.ld.q[row][c8]) = vq;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int kk = 0; kk < MX_KC; kk += 16) {
+      uint32_t bf[4][2];
+#pragma unroll
+      for (int p = 0; p < 2; p++) {
+        uint32_t t[4];
+        ldsm_x4(t, &sm.ld.q[kk + (lane & 15)][wn * 32 + p * 16 + (lane >> 4) * 8], true);
+        bf[2 * p][0] = t[0]; bf[2 * p][1] = t[1]; bf[2 * p + 1][0] = t[2]; bf[2 * p + 1][1] = t[3];
+      }
+#pragma unroll
+      for (int mt = 0; mt < 4; mt++) {
+        uint32_t ah[4], al[4];
+        const int row = wm * 64 + mt * 16 + (lane & 15), col = kk + (lane >> 4) * 8;
+        ldsm_x4(ah, &sm.ld.a_hi[row][col], false);
+        ldsm_x4(al, &sm.ld.a_lo[row][col], false);
+#pragma unroll
+        for (int nt = 0; nt < 4; nt++) {
+          mma_f16(acc[mt][nt], al, bf[nt]);
+          mma_f16(acc[mt][nt], ah, bf[nt]);
+        }
+      }
+    }
+    __syncthreads();
+  }
+
+#pragma unroll
+  for (int mt = 0; mt < 4; mt++)
+#pragma unroll
+    for (int nt = 0; nt < 4; nt++) {
+      const int r = wm * 64 + mt * 16 + (lane >> 2), c = wn * 32 + nt * 8 + (lane & 3) * 2;
+      const float u = 1.f / MX_WSCALE;
+      *reinterpret_cast<__half2*>(&sm.out[r][c]) = __floats2half2_rn(acc[mt][nt][0] * u, acc[mt][nt][1] * u);
+      *reinterpret_cast<__half2*>(&sm.out[r + 8][c]) = __floats2half2_rn(acc[mt][nt][2] * u, acc[mt][nt][3] * u);
+    }
+  __syncthreads();
+#pragma unroll
+  for (int u = 0; u < MX_BM * MX_BN / 8 / MX_T; u++) {  // whole 16-byte row segments
+    const int idx = tid + u * MX_T, row = idx >> 4, c8 = (idx & 15) * 8;
+    const long long gr = m0 + row;
+    const int gk = n0 + c8;
+    if (gr < R && gk < K) *reinterpret_cast<uint4*>(out + gr * K + gk) = *reinterpret_cast<const uint4*>(&sm.out[row][c8]);
+  }
+}
+
 }  // namespace
 
 ESVIT_API int esvit_row_lse(const void* x, const float* center, float inv_temp, float* lse, long long R, int K,
@@ -560,6 +704,22 @@ ESVIT_API int esvit_dino_ce_q_bwd(const void* s, const void* q, const float* lse
   if (K % 8 != 0 || R <= 0) return ESVIT_ERR_BAD_ARG;
   dino_ce_q_bwd_kernel<<<(unsigned)R, LT, 0, (cudaStream_t)stream>>>((const bf16*)s, (const half8*)q, lse_s, trow, w, gscale,
                                                                      inv_tau_s, (bf16*)ds, K, order);
+  ESVIT_LAUNCH_CHECK();
+}
+
+// ---- mixup targets (see mixup_q_kernel) ----
+ESVIT_API int esvit_mixup_q_kpad(int B) { return (2 * B + MX_KC - 1) / MX_KC * MX_KC; }
+
+ESVIT_API int esvit_mixup_q(const float* targets, const void* q, int ncrops, int B, int K, float w_scale, void* ws,
+                            float* w, void* q_out, void* stream) {
+  if (K % 8 != 0 || K <= 0 || B <= 0 || ncrops < 2 || (long long)ncrops * B > (1LL << 30)) return ESVIT_ERR_BAD_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int R = ncrops * B, Kp = esvit_mixup_q_kpad(B);
+  __half* a_hi = (__half*)ws;
+  __half* a_lo = a_hi + (long long)R * Kp;
+  mixup_weights_kernel<<<(unsigned)((R + 7) / 8), 256, 0, st>>>(targets, ncrops, B, Kp, w_scale, a_hi, a_lo, w);
+  mixup_q_kernel<<<dim3((K + MX_BN - 1) / MX_BN, (R + MX_BM - 1) / MX_BM), MX_T, 0, st>>>(
+      a_hi, a_lo, (const __half*)q, (__half*)q_out, R, 2 * B, K, Kp);
   ESVIT_LAUNCH_CHECK();
 }
 

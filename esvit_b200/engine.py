@@ -18,7 +18,7 @@ import torch.nn as nn
 import torch.distributed as dist
 
 from . import ops, utils
-from .losses import DDINOLoss, DINOLoss
+from .losses import DDINOLoss, DINOLoss, mixup_targets
 from .optim import FusedAdamWEMA
 from . import cvt_v4_transformer as cvts
 from . import vision_longformer as vils
@@ -159,6 +159,8 @@ class SelfDistillStep:
         self._static_in = None
         self._static_loss = None
         self._warm = 0
+        self._static_mix = None  # (teacher crops, student crops, targets) of the student_images / targets_mixup step
+        self._warm_mix = 0
         for p in self.teacher.parameters():
             p.requires_grad = False
         # arena for the ACCUMULATED small gradients (LN affine, biases, rel-pos tables, patch embed): sized from the model
@@ -169,11 +171,12 @@ class SelfDistillStep:
             self._reducer = _GradReducer(list(self.student.parameters()))
 
     # ---- the step body (eager; also what gets captured) ---------------------------------------------------
-    def _body(self, images: List[torch.Tensor], epoch: int) -> torch.Tensor:
+    def _body(self, images: List[torch.Tensor], epoch: int, student_images: Optional[List[torch.Tensor]] = None,
+              targets_mixup: Optional[List[torch.Tensor]] = None) -> torch.Tensor:
         with torch.no_grad():
             teacher_output = self.teacher(images[:2])
-        student_output = self.student_call(images)
-        loss = self.loss(student_output, teacher_output, epoch, None)
+        student_output = self.student_call(images if student_images is None else student_images)
+        loss = self.loss(student_output, teacher_output, epoch, targets_mixup)
         if self.fused:
             self.opt.zero_grad()
         else:
@@ -201,7 +204,16 @@ class SelfDistillStep:
             self._reducer.finish()
 
     def __call__(self, images: Sequence[torch.Tensor], epoch: int, lr: float, wd: float, momentum: float) -> torch.Tensor:
+        return self.step(images, epoch, lr, wd, momentum)
+
+    def step(self, images: Sequence[torch.Tensor], epoch: int, lr: float, wd: float, momentum: float,
+             student_images: Optional[Sequence[torch.Tensor]] = None,
+             targets_mixup: Optional[Sequence[torch.Tensor]] = None) -> torch.Tensor:
+        """One step.  The teacher reads images[:2]; the student reads student_images when given (the mixed crops of
+        ``--use_mixup``, main_esvit.py:516-543), else images; targets_mixup goes to the loss (per-view [B, B] targets)."""
         images = list(images)
+        student_images = None if student_images is None else list(student_images)
+        targets_mixup = list(targets_mixup) if targets_mixup else None
         if self.fused:
             self.opt.set_hyper(lr, wd, momentum)
             self.opt.set_skip_last_layer(epoch < self.freeze_last_layer)
@@ -211,11 +223,13 @@ class SelfDistillStep:
                 if i == 0:
                     g["weight_decay"] = wd
         if not self.use_cuda_graph:
-            loss = self._body(images, epoch)
+            loss = self._body(images, epoch, student_images, targets_mixup)
             if not self.fused:
                 utils.ema_update(self.student, self.teacher, momentum)
             return loss
-        return self._graphed(images, epoch)
+        if student_images is None and targets_mixup is None:
+            return self._graphed(images, epoch)
+        return self._graphed_mixup(images, epoch, images if student_images is None else student_images, targets_mixup)
 
     # ---- CUDA-graph path ------------------------------------------------------------------------------------
     def _graphed(self, images: List[torch.Tensor], epoch: int) -> torch.Tensor:
@@ -223,17 +237,8 @@ class SelfDistillStep:
         caller's crops into them on the current stream, so the caller may recycle its own (prefetch) buffers freely.  A
         batch of a different shape (e.g. a shorter last batch) runs the eager body instead."""
         if self._static_in is None:
-            # crops of one shape share one buffer, back to back: the multi-crop forward then views a resolution group
-            # as one batch instead of concatenating it (ops.cat_adjacent)
-            self._static_in, i = [], 0
-            while i < len(images):
-                j = i
-                while j < len(images) and images[j].shape == images[i].shape and images[j].dtype == images[i].dtype:
-                    j += 1
-                buf = torch.empty((j - i,) + tuple(images[i].shape), dtype=images[i].dtype, device=images[i].device)
-                self._static_in += [buf[k] for k in range(j - i)]
-                i = j
-        if len(images) != len(self._static_in) or any(s.shape != im.shape for s, im in zip(self._static_in, images)):
+            self._static_in = _static_buffers(images)
+        if not _fits(self._static_in, images):
             return self._body(images, epoch)
         for s, im in zip(self._static_in, images):
             s.copy_(im, non_blocking=True)
@@ -252,6 +257,60 @@ class SelfDistillStep:
             ent = self._graphs[key] = (g, out)
         ent[0].replay()
         return ent[1]
+
+    def _graphed_mixup(self, images: List[torch.Tensor], epoch: int, student_images: List[torch.Tensor],
+                       targets_mixup: Optional[List[torch.Tensor]]) -> torch.Tensor:
+        """Replay path of a step with student_images / targets_mixup: its own graph per (teacher_temp, last-layer-frozen)
+        state, reading private static buffers for the two teacher crops, the student crops and the targets.  The targets
+        are checked (losses.mixup_targets) before they are copied in; inside the capture only their shape is."""
+        if targets_mixup is not None:
+            B = images[0].shape[0]
+            targets = mixup_targets(targets_mixup, self.loss.ncrops, B, images[0].device)
+        if self._static_mix is None:
+            self._static_mix = (_static_buffers(images[:2]), _static_buffers(student_images),
+                                None if targets_mixup is None else torch.empty_like(targets))
+        st_t, st_s, st_y = self._static_mix
+        if (not _fits(st_t, images[:2]) or not _fits(st_s, student_images) or (st_y is None) != (targets_mixup is None)
+                or (st_y is not None and st_y.shape != targets.shape)):
+            return self._body(images, epoch, student_images, targets_mixup)
+        for s, im in zip(st_t + st_s, images[:2] + student_images):
+            s.copy_(im, non_blocking=True)
+        if st_y is not None:
+            st_y.copy_(targets, non_blocking=True)
+        args = (st_t, epoch, st_s, None if st_y is None else list(st_y.unbind(0)))
+        if self._warm_mix < 3:
+            self._warm_mix += 1
+            return self._body(*args)
+        key = (float(self.loss.teacher_temp_schedule[epoch]), epoch < self.freeze_last_layer, "mixup")
+        ent = self._graphs.get(key)
+        if ent is None:
+            torch.cuda.synchronize()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, pool=self._pool):
+                out = self._body(*args)
+            if self._pool is None:
+                self._pool = g.pool()
+            ent = self._graphs[key] = (g, out)
+        ent[0].replay()
+        return ent[1]
+
+
+def _static_buffers(images: List[torch.Tensor]) -> List[torch.Tensor]:
+    """Views of private buffers shaped like `images`.  Crops of one shape share one buffer, back to back: the multi-crop
+    forward then views a resolution group as one batch instead of concatenating it (ops.cat_adjacent)."""
+    out, i = [], 0
+    while i < len(images):
+        j = i
+        while j < len(images) and images[j].shape == images[i].shape and images[j].dtype == images[i].dtype:
+            j += 1
+        buf = torch.empty((j - i,) + tuple(images[i].shape), dtype=images[i].dtype, device=images[i].device)
+        out += [buf[k] for k in range(j - i)]
+        i = j
+    return out
+
+
+def _fits(static: List[torch.Tensor], images: List[torch.Tensor]) -> bool:
+    return len(images) == len(static) and all(s.shape == im.shape for s, im in zip(static, images))
 
 
 def make_step(arch: str = "swin_tiny_w7", out_dim: int = 65536, ncrops: int = 10, dense: bool = True,

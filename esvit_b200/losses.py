@@ -1,6 +1,7 @@
 """DINOLoss / DDINOLoss behind the reference's constructor + call signatures (main_esvit.py:603-770).
 
-``loss(student_output, teacher_output, epoch, targets_mixup) -> 0-dim tensor``; buffers ``center`` (and
+``loss(student_output, teacher_output, epoch, targets_mixup) -> 0-dim tensor``: DINOLoss weights its terms by the
+mixup targets when they are given (``--use_mixup``), DDINOLoss ignores them like the reference's; buffers ``center`` (and
 ``center_grid``) [1, out_dim] live in ``state_dict()`` like the reference's.
 
 Fused formulation (DESIGN.md): one streaming pass per student row over its <= 2 paired teacher rows
@@ -91,14 +92,42 @@ class _CenteredLoss(nn.Module):
         return center.detach().view(-1).clone()
 
 
+def mixup_targets(targets_mixup, ncrops: int, B: int, device) -> torch.Tensor:
+    """The per-view soft targets of main_esvit.py:515-544 (timm's ``mixup_fn`` targets, or ``torch.eye(B)`` for views
+    past ``num_mixup_views``) as one fp32 [ncrops, B, B] tensor.  Raises ValueError unless they are a list of ``ncrops``
+    floating [B, B] tensors on ``device`` with finite, non-negative values.  The value check reads one flag on the host;
+    it is skipped while a CUDA graph is being captured (engine.SelfDistillStep checks the values it copies in)."""
+    if not isinstance(targets_mixup, (list, tuple)) or len(targets_mixup) != ncrops:
+        raise ValueError(f"targets_mixup must be a list of {ncrops} [B, B] tensors (one per view)")
+    for v, t in enumerate(targets_mixup):
+        if not isinstance(t, torch.Tensor) or not t.is_floating_point() or tuple(t.shape) != (B, B):
+            raise ValueError(f"targets_mixup[{v}] must be a floating [{B}, {B}] tensor, got "
+                             f"{tuple(t.shape) if isinstance(t, torch.Tensor) else type(t).__name__}")
+        if t.device != torch.device(device):
+            raise ValueError(f"targets_mixup[{v}] is on {t.device}, the logits on {device}")
+    T = torch.stack([t.detach().float() for t in targets_mixup])
+    if not torch.cuda.is_current_stream_capturing():
+        check_mixup_values(T)
+    return T
+
+
+def check_mixup_values(T: torch.Tensor) -> None:
+    """ValueError unless every target is finite and non-negative (one host read when they are)."""
+    if not bool((torch.isfinite(T) & (T >= 0)).all()):
+        bad = "non-finite" if not bool(torch.isfinite(T).all()) else "negative"
+        raise ValueError(f"targets_mixup has {bad} entries; mixup targets are finite, non-negative weights")
+
+
 class DINOLoss(_CenteredLoss):
     def forward(self, student_output, teacher_output, epoch, targets_mixup=None):
-        if targets_mixup:
-            raise NotImplementedError("mixup targets (main_esvit.py:638-640) are outside the hot-path scope")
         s, t = self._as_bf16(student_output), self._as_bf16(teacher_output).detach()
         B = t.shape[0] // 2
         temp = float(self.teacher_temp_schedule[epoch])
         n_terms = 2 * self.ncrops - 2
+        if isinstance(targets_mixup, torch.Tensor) or targets_mixup:  # (a tensor is rejected by mixup_targets)
+            loss = self._mixup_loss(s, t, targets_mixup, B, temp, n_terms)
+            self.update_center(t)
+            return loss
         trow, w = self._cls_tables(B, 1.0 / (n_terms * B), s.device)
         center = self._snapshot(self.center)
         lse_t = None if ops.ce_q_enabled(t.shape[-1]) else ops.row_lse(t, center, 1.0 / temp)
@@ -106,6 +135,22 @@ class DINOLoss(_CenteredLoss):
                                   self._order(B, [(self.ncrops, 1)], s.device))
         self.update_center(t)
         return loss
+
+    def _mixup_loss(self, s, t, targets_mixup, B, temp, n_terms):
+        """main_esvit.py:638-641: every (iq, v != iq) term is -mean_j sum_b T_v[j, b] <q^iq_j, log_softmax(s_{v,b})>.
+        Both global views fold into one mixed teacher row per student row (ops.mixup_q), paired with that row alone."""
+        K = t.shape[-1]
+        if not ops.ce_q_enabled(K):
+            raise NotImplementedError("mixup targets run on the stored teacher probabilities only "
+                                      f"(ESVIT_CE_Q=0, or out_dim {K} > esvit_row_softmax_q_max_k)")
+        T = mixup_targets(targets_mixup, self.ncrops, B, s.device)
+        _, q = ops.row_softmax_q(t, self.center.view(-1), 1.0 / temp)
+        q_hat, w = ops.mixup_q(q, T, 1.0 / (n_terms * B))
+        key = ("self", s.shape[0], str(s.device))
+        if key not in self._tables:
+            r = torch.arange(s.shape[0], dtype=torch.int32)
+            self._tables[key] = (torch.stack([r, torch.full_like(r, -1)], 1).contiguous().to(s.device), None)
+        return ops.DinoCEQFn.apply(s, q_hat, self._tables[key][0], w, 1.0 / self.student_temp)
 
     @torch.no_grad()
     def update_center(self, teacher_output):
@@ -128,8 +173,7 @@ class DDINOLoss(_CenteredLoss):
         return self._tables[key][1]
 
     def forward(self, student_output, teacher_output, epoch, targets_mixup=None):
-        if targets_mixup:
-            raise NotImplementedError("mixup targets are outside the hot-path scope")
+        """targets_mixup is accepted and ignored, as the reference's DDINOLoss does (main_esvit.py:683-750)."""
         s_cls_out, s_region_out, s_fea, s_npatch = student_output
         t_cls_out, t_region_out, t_fea, t_npatch = teacher_output
         s_cls, s_reg = self._as_bf16(s_cls_out), self._as_bf16(s_region_out)

@@ -931,6 +931,27 @@ def row_softmax_q(x: Tensor, center: Tensor, inv_temp: float) -> Tuple[Tensor, T
     return lse, q
 
 
+def _ce_q_fwd(s: Tensor, q: Tensor, trow: Tensor, order: Optional[Tensor], w: Tensor,
+              inv_tau_s: float) -> Tuple[Tensor, Tensor]:
+    """(loss = sum_r w[r] * row_loss[r], lse_s) of esvit_dino_ce_q_fwd on stored teacher probabilities q."""
+    R, K = s.shape
+    lse_s = torch.empty(R, dtype=F32, device=s.device)  # written by the CE kernel itself (one pass over s)
+    row_loss = torch.empty(R, dtype=F32, device=s.device)
+    _lib.call("esvit_dino_ce_q_fwd", _p(s), _p(q), _p(lse_s), _p(trow), _p(order), inv_tau_s, _p(row_loss), R, K,
+              _stream())
+    loss = torch.empty((), dtype=F32, device=s.device)
+    _lib.call("esvit_weighted_sum", _p(row_loss), _p(w), R, _p(loss), _stream())
+    return loss, lse_s
+
+
+def _ce_q_bwd(s, q, lse_s, trow, w, order, gs, inv_tau_s: float) -> Tensor:
+    R, K = s.shape
+    ds = torch.empty_like(s)
+    _lib.call("esvit_dino_ce_q_bwd", _p(s), _p(q), _p(lse_s), _p(trow), _p(order), _p(w), _p(gs), inv_tau_s, _p(ds),
+              R, K, _stream())
+    return ds
+
+
 class DinoCEFn(Function):
     """loss = sum_r w[r] * ( n_r * LSE(s_r / tau) - sum_j <softmax((t[trow[r,j]] - center) / temp), s_r / tau> ).
 
@@ -945,23 +966,22 @@ class DinoCEFn(Function):
         center, w = _chk(center, F32, "center"), _chk(w, F32, "w")
         trow = _chk(trow, torch.int32, "trow")
         order = _chk(order, torch.int32, "order")
+        ctx.use_q = lse_t is None
+        ctx.temps = (inv_temp_t, inv_tau_s)
+        if ctx.use_q:
+            _, q = row_softmax_q(t, center, inv_temp_t)
+            loss, lse_s = _ce_q_fwd(s, q, trow, order, w, inv_tau_s)
+            ctx.save_for_backward(s, q, lse_s, trow, w, order)
+            return loss
         R, K = s.shape
         lse_s = torch.empty(R, dtype=F32, device=s.device)  # written by the CE kernel itself (one pass over s)
         row_loss = torch.empty(R, dtype=F32, device=s.device)
-        ctx.use_q = lse_t is None
-        if ctx.use_q:
-            _, q = row_softmax_q(t, center, inv_temp_t)
-            _lib.call("esvit_dino_ce_q_fwd", _p(s), _p(q), _p(lse_s), _p(trow), _p(order), inv_tau_s, _p(row_loss), R, K,
-                      _stream())
-            ctx.save_for_backward(s, q, lse_s, trow, w, order)
-        else:
-            lse_t = _chk(lse_t, F32, "lse_t")
-            _lib.call("esvit_dino_ce_fwd", _p(s), _p(t), _p(center), _p(lse_s), _p(lse_t), _p(trow), _p(order), inv_temp_t,
-                      inv_tau_s, _p(row_loss), R, K, _stream())
-            ctx.save_for_backward(s, t, center, lse_s, lse_t, trow, w, order)
+        lse_t = _chk(lse_t, F32, "lse_t")
+        _lib.call("esvit_dino_ce_fwd", _p(s), _p(t), _p(center), _p(lse_s), _p(lse_t), _p(trow), _p(order), inv_temp_t,
+                  inv_tau_s, _p(row_loss), R, K, _stream())
+        ctx.save_for_backward(s, t, center, lse_s, lse_t, trow, w, order)
         loss = torch.empty((), dtype=F32, device=s.device)
         _lib.call("esvit_weighted_sum", _p(row_loss), _p(w), R, _p(loss), _stream())
-        ctx.temps = (inv_temp_t, inv_tau_s)
         return loss
 
     @staticmethod
@@ -970,11 +990,7 @@ class DinoCEFn(Function):
         inv_temp_t, inv_tau_s = ctx.temps
         gs = _chk(g.reshape(1).to(F32), F32, "g")
         if ctx.use_q:
-            s, q, lse_s, trow, w, order = ctx.saved_tensors
-            R, K = s.shape
-            ds = torch.empty_like(s)
-            _lib.call("esvit_dino_ce_q_bwd", _p(s), _p(q), _p(lse_s), _p(trow), _p(order), _p(w), _p(gs), inv_tau_s, _p(ds),
-                      R, K, _stream())
+            ds = _ce_q_bwd(*ctx.saved_tensors, gs, inv_tau_s)
         else:
             s, t, center, lse_s, lse_t, trow, w, order = ctx.saved_tensors
             R, K = s.shape
@@ -982,6 +998,43 @@ class DinoCEFn(Function):
             _lib.call("esvit_dino_ce_bwd", _p(s), _p(t), _p(center), _p(lse_s), _p(lse_t), _p(trow), _p(order), _p(w),
                       _p(gs), inv_temp_t, inv_tau_s, _p(ds), R, K, _stream())
         return ds, None, None, None, None, None, None, None, None
+
+
+def mixup_q(q: Tensor, targets: Tensor, w_scale: float) -> Tuple[Tensor, Tensor]:
+    """Mixed teacher rows of the mixup loss (esvit_mixup_q): q fp16 [2B, K] from row_softmax_q, targets fp32
+    [ncrops, B, B] (finite, non-negative) -> (q_hat fp16 [ncrops*B, K] in the same format, w fp32 [ncrops*B])."""
+    q, targets = _chk(q, torch.float16, "teacher probabilities"), _chk(targets, F32, "mixup targets")
+    ncrops, B, B2 = targets.shape
+    Rt, K = q.shape
+    if B2 != B or Rt != 2 * B:
+        raise ValueError(f"mixup targets {tuple(targets.shape)} do not fit {Rt} teacher rows")
+    R = ncrops * B
+    ws = torch.empty(2 * R * _lib.load().esvit_mixup_q_kpad(B), dtype=torch.float16, device=q.device)
+    w = torch.empty(R, dtype=F32, device=q.device)
+    q_hat = torch.empty(R, K, dtype=torch.float16, device=q.device)
+    _lib.call("esvit_mixup_q", _p(targets), _p(q), ncrops, B, K, w_scale, _p(ws), _p(w), _p(q_hat), _stream())
+    return q_hat, w
+
+
+class DinoCEQFn(Function):
+    """loss = sum_r w[r] * ( n_r * LSE(s_r / tau) - sum_j <q[trow[r,j]] / 2^12, s_r / tau> ) on stored teacher
+    probabilities q (fp16, the row_softmax_q / mixup_q format); w is read on the device, gradient to s only."""
+
+    @staticmethod
+    def forward(ctx, s, q, trow, w, inv_tau_s: float):
+        s, q = _chk(s, BF16, "student logits"), _chk(q, torch.float16, "teacher probabilities")
+        trow, w = _chk(trow, torch.int32, "trow"), _chk(w, F32, "w")
+        loss, lse_s = _ce_q_fwd(s, q, trow, None, w, inv_tau_s)
+        ctx.save_for_backward(s, q, lse_s, trow, w)
+        ctx.inv_tau_s = inv_tau_s
+        return loss
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        s, q, lse_s, trow, w = ctx.saved_tensors
+        gs = _chk(g.reshape(1).to(F32), F32, "g")
+        return _ce_q_bwd(s, q, lse_s, trow, w, None, gs, ctx.inv_tau_s), None, None, None, None
 
 
 _colsum_ws = {}

@@ -169,6 +169,16 @@ int esvit_dino_ce_q_fwd(const void* s, const void* q, float* lse_s, const int* t
                         float* row_loss, long long R, int K, void* stream);
 int esvit_dino_ce_q_bwd(const void* s, const void* q, const float* lse_s, const int* trow, const int* order,
                         const float* w, const float* gscale, float inv_tau_s, void* ds, long long R, int K, void* stream);
+/* Mixup targets (main_esvit.py:638-641): targets fp32 [ncrops, B, B] (T_v[j, b], teacher sample j, student sample b),
+ * finite and non-negative; q the fp16 [2B, K] output of esvit_row_softmax_q.  For student row r = (v, b):
+ *   C_r = sum_{iq != v} sum_j T_v[j, b],   q_out[r] = sum_{iq != v} sum_j T_v[j, b] * q[iq*B + j] / C_r  (0 where C_r = 0)
+ *   w[r] = C_r * w_scale
+ * so esvit_dino_ce_q_fwd / bwd on q_out with trow[r] = (r, -1) and this w compute the mixup loss when w_scale =
+ * 1 / (n_terms * B).  q_out fp16 [ncrops*B, K] in the same 2^12-scaled format; ws: fp16 [2 * ncrops*B *
+ * esvit_mixup_q_kpad(B)] scratch. */
+int esvit_mixup_q_kpad(int B);
+int esvit_mixup_q(const float* targets, const void* q, int ncrops, int B, int K, float w_scale, void* ws, float* w,
+                  void* q_out, void* stream);
 
 /* ---- update_center ----------------------------------------------------------- main_esvit.py:650-660, :752-770
  * colsum: out[k] = sum_r t[r,k] (deterministic two-stage); workspace fp32 [esvit_colsum_workspace_rows()*K].
