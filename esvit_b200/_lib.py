@@ -71,6 +71,10 @@ SIGNATURES = {
     "esvit_dwbn_fwd_apply": [P, P, P, P, P, P, P, P, P, L, I, I, F, F, P],
     "esvit_dwbn_bwd_stats": [P, P, P, P, P, P, P, L, I, P],
     "esvit_dwbn_bwd_apply": [P, P, P, P, P, P, P, P, P, P, I, I, I, I, I, I, I, P],
+    "esvit_headbn_fwd_stats": [P, P, P, L, I, P],
+    "esvit_headbn_fwd_apply": [P, P, P, P, P, P, P, P, P, L, I, I, F, F, P],
+    "esvit_headbn_bwd_stats": [P, P, P, P, P, P, P, L, I, P],
+    "esvit_headbn_bwd_apply": [P, P, P, P, P, P, P, P, L, I, I, P],
     "esvit_vil_sc_ws_floats": [I, I, I, I],
     "esvit_vil_sc_fwd": [P, P, P, P, P, P, P, P, I, I, I, I, F, P],
     "esvit_vil_sc_bwd": [P, P, P, P, P, P, P, P, P, P, P, P, P, P, P, I, I, I, I, F, P],
@@ -148,7 +152,9 @@ def call(name: str, *args) -> None:
 # ---- instrumentation used by bench.py (launch counting; live CUDA-event timing of one entry point) --------------
 # kernels launched per call of each entry point (entries that launch more than one kernel are computed per call)
 _LAUNCHES = {"esvit_colsum": 2, "esvit_gemm_mul_colsum": 2, "esvit_gemm_mul_colsum2": 2, "esvit_gemm_wgrad": 2,
-             "esvit_mixup_q": 2}  # GEMM + fold; mixup weights + product
+             "esvit_mixup_q": 2,  # GEMM + fold; mixup weights + product
+             "esvit_headbn_fwd_stats": 2, "esvit_headbn_fwd_apply": 2, "esvit_headbn_bwd_stats": 2,
+             "esvit_headbn_bwd_apply": 3}
 _launch_count = 0
 _timed_names = set()
 _timed_events = []
@@ -181,6 +187,10 @@ _META = {
                                        "C": int(a[10])},
     "esvit_dwbn_fwd_apply": lambda a: {"N": int(a[9]), "C": int(a[10])},
     "esvit_dwbn_bwd_stats": lambda a: {"N": int(a[7]), "C": int(a[8])},
+    "esvit_headbn_fwd_stats": lambda a: {"N": int(a[3]), "C": int(a[4])},
+    "esvit_headbn_fwd_apply": lambda a: {"N": int(a[9]), "C": int(a[10])},
+    "esvit_headbn_bwd_stats": lambda a: {"N": int(a[7]), "C": int(a[8])},
+    "esvit_headbn_bwd_apply": lambda a: {"N": int(a[8]), "C": int(a[9])},
     "esvit_dwbn_bwd_apply": lambda a: {"B": int(a[10]), "H": int(a[11]), "W": int(a[12]), "Hp": int(a[13]),
                                        "Wp": int(a[14]), "C": int(a[15])},
     "esvit_mhsa_win_fwd": lambda a: {"B": int(a[3]), "H": int(a[4]), "W": int(a[5]), "w": int(a[6]), "C": int(a[7]),

@@ -1,5 +1,7 @@
 // CvT-specific kernels (models/cvt_v4_transformer.py): the convolutional token embedding's patch gather and its
-// transpose, and the depthwise 3x3 conv + BatchNorm2d in front of the qkv projection, forward and backward.
+// transpose, and the depthwise 3x3 conv + BatchNorm2d in front of the qkv projection, forward and backward.  The
+// BatchNorm1d + GELU of a DINOHead(use_bn=True) (models/vision_transformer.py:389-397) shares their statistics, running-
+// statistics and coefficient arithmetic (esvit_headbn_*, at the end of this file).
 //
 // Conv embed (ConvEmbed :349-382): Conv2d(k, stride, pad) = im2col rows bf16 [B*Ho*Wo, Kp] in the weight's (c, ky, kx)
 // order (columns >= Cin*k*k are zero, Kp % 8 == 0 for the TMA row pitch) + the bias-epilogue GEMM.  The input is the fp32
@@ -197,6 +199,7 @@ __global__ void bn_finalize_kernel(const double* __restrict__ sums, const float*
   stat[3 * C + c] = beta[c] - (float)mean * sc;
 }
 
+template <bool GELU>
 __global__ void bn_normalize_kernel(const bf16* __restrict__ z, const float* __restrict__ stat, bf16* __restrict__ out,
                                     int C, long long n8) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
@@ -204,23 +207,34 @@ __global__ void bn_normalize_kernel(const bf16* __restrict__ z, const float* __r
     float f[8];
     unpack8(reinterpret_cast<const bf16x8*>(z)[i], f);
 #pragma unroll
-    for (int q = 0; q < 8; q++) f[q] = fmaf(f[q], stat[2 * C + c0 + q], stat[3 * C + c0 + q]);
+    for (int q = 0; q < 8; q++) {
+      f[q] = fmaf(f[q], stat[2 * C + c0 + q], stat[3 * C + c0 + q]);
+      if (GELU) f[q] = gelu_f(f[q]);
+    }
     reinterpret_cast<bf16x8*>(out)[i] = pack8(f);
   }
 }
 
+// gradient at the BN output: dy, or (GELU) dy * gelu'(z scale + shift) for the BN + GELU of the DINO head
+template <bool GELU>
+__device__ __forceinline__ float bn_dout(float dy, float z, float sc, float sh) {
+  return GELU ? dy * gelu_grad_f(fmaf(z, sc, sh)) : dy;
+}
+
 // partials of (sum dy, sum dy * xhat) per channel
+template <bool GELU>
 __global__ void __launch_bounds__(NT) bn_bwd_partials_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ z,
                                                              const float* __restrict__ stat, float* __restrict__ part,
                                                              long long N, int C) {
   const int tx = threadIdx.x & 63, ty = threadIdx.x >> 6, c = blockIdx.y * 64 + tx;
-  const float mean = stat[c], rstd = stat[C + c];
+  const float mean = stat[c], rstd = stat[C + c], sc = stat[2 * C + c], sh = stat[3 * C + c];
   float v[2] = {0.f, 0.f};
   const long long p0 = (long long)blockIdx.x * PCH;
   for (int i = ty; i < PCH; i += 4) {
     const long long p = p0 + i;
     if (p >= N) break;
-    const float g = ld(dy + p * C + c), xh = (ld(z + p * C + c) - mean) * rstd;
+    const float zv = ld(z + p * C + c);
+    const float g = bn_dout<GELU>(ld(dy + p * C + c), zv, sc, sh), xh = (zv - mean) * rstd;
     v[0] += g;
     v[1] = fmaf(g, xh, v[1]);
   }
@@ -291,6 +305,44 @@ __global__ void __launch_bounds__(NT) dw_bwd_w_kernel(const bf16* __restrict__ d
     for (int t = 0; t < 9; t++) v[t] = fmaf(d, ypad(y, g, b, py + t / 3 - 1, px + t % 3 - 1, c), v[t]);
   }
   block_partials<9>(v, part, g.C);
+}
+
+// DINO head BN: per-column sums of z bf16 [N, C] (the bias-GEMM output) and of z^2
+__global__ void __launch_bounds__(NT) head_stats_kernel(const bf16* __restrict__ z, float* __restrict__ part, long long N,
+                                                        int C) {
+  const int tx = threadIdx.x & 63, ty = threadIdx.x >> 6, c = blockIdx.y * 64 + tx;
+  float v[2] = {0.f, 0.f};
+  const long long p0 = (long long)blockIdx.x * PCH;
+  for (int i = ty; i < PCH; i += 4) {
+    const long long p = p0 + i;
+    if (p >= N) break;
+    const float zv = ld(z + p * C + c);
+    v[0] += zv;
+    v[1] = fmaf(zv, zv, v[1]);
+  }
+  block_partials<2>(v, part, C);
+}
+
+// DINO head BN backward: dz = coef0 gelu'(u) dy + coef1 z + coef2 (bf16, the GEMM operand of dx / dW) and the partials
+// of its column sums (the gradient of the Linear's bias)
+__global__ void __launch_bounds__(NT) head_bwd_dz_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ z,
+                                                         const float* __restrict__ stat, const float* __restrict__ coef,
+                                                         bf16* __restrict__ dz, float* __restrict__ part, long long N,
+                                                         int C) {
+  const int tx = threadIdx.x & 63, ty = threadIdx.x >> 6, c = blockIdx.y * 64 + tx;
+  const float sc = stat[2 * C + c], sh = stat[3 * C + c];
+  const float c0 = coef[c], c1 = coef[C + c], c2 = coef[2 * C + c];
+  float v[1] = {0.f};
+  const long long p0 = (long long)blockIdx.x * PCH;
+  for (int i = ty; i < PCH; i += 4) {
+    const long long p = p0 + i;
+    if (p >= N) break;
+    const float zv = ld(z + p * C + c);
+    const float d = fmaf(c0, bn_dout<true>(ld(dy + p * C + c), zv, sc, sh), fmaf(c1, zv, c2));
+    dz[p * C + c] = __float2bfloat16(d);
+    v[0] += d;
+  }
+  block_partials<1>(v, part, C);
 }
 
 static unsigned grid_for(long long total, int threads) {
@@ -368,7 +420,7 @@ ESVIT_API int esvit_dwbn_fwd_apply(const void* z, const float* gamma, const floa
   cvt::bn_finalize_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, gamma, beta, run_mean, run_var, nbt, stat, C, train,
                                                            momentum, eps);
   const long long n8 = N * C / 8;
-  cvt::bn_normalize_kernel<<<cvt::grid_for(n8, 256), 256, 0, st>>>((const bf16*)z, stat, (bf16*)out, C, n8);
+  cvt::bn_normalize_kernel<false><<<cvt::grid_for(n8, 256), 256, 0, st>>>((const bf16*)z, stat, (bf16*)out, C, n8);
   ESVIT_LAUNCH_CHECK();
 }
 
@@ -378,8 +430,8 @@ ESVIT_API int esvit_dwbn_bwd_stats(const void* dy, const void* z, const float* s
   cudaStream_t st = (cudaStream_t)stream;
   const long long nchunk = (N + cvt::PCH - 1) / cvt::PCH;
   if (nchunk >= (1LL << 31)) return ESVIT_ERR_BAD_ARG;
-  cvt::bn_bwd_partials_kernel<<<dim3((unsigned)nchunk, C / 64), cvt::NT, 0, st>>>((const bf16*)dy, (const bf16*)z, stat,
-                                                                                 part, N, C);
+  cvt::bn_bwd_partials_kernel<false><<<dim3((unsigned)nchunk, C / 64), cvt::NT, 0, st>>>((const bf16*)dy, (const bf16*)z,
+                                                                                        stat, part, N, C);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return (int)e;
   return (int)cvt::fold(part, nchunk, 2, C, sums, (double)N, dbeta, dgamma, nullptr, st);
@@ -403,4 +455,60 @@ ESVIT_API int esvit_dwbn_bwd_apply(const void* dy, const void* z, const void* y,
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return (int)e;
   return (int)cvt::fold(part, nchunk, 9, C, nullptr, 0.0, nullptr, nullptr, dw, st);
+}
+
+// ---- DINOHead(use_bn=True): Linear -> BatchNorm1d -> GELU on rows z bf16 [N, C] (the bias-GEMM output) ----------------
+
+static bool head_ok(long long N, int C) {
+  return N >= 1 && C >= 64 && C % 64 == 0 && (N + cvt::PCH - 1) / cvt::PCH < (1LL << 31);
+}
+
+ESVIT_API int esvit_headbn_fwd_stats(const void* z, float* part, double* sums, long long N, int C, void* stream) {
+  if (!z || !part || !sums || !head_ok(N, C)) return ESVIT_ERR_BAD_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long nchunk = (N + cvt::PCH - 1) / cvt::PCH;
+  cvt::head_stats_kernel<<<dim3((unsigned)nchunk, C / 64), cvt::NT, 0, st>>>((const bf16*)z, part, N, C);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return (int)e;
+  return (int)cvt::fold(part, nchunk, 2, C, sums, (double)N, nullptr, nullptr, nullptr, st);
+}
+
+ESVIT_API int esvit_headbn_fwd_apply(const void* z, const float* gamma, const float* beta, const double* sums,
+                                     float* run_mean, float* run_var, long long* nbt, float* stat, void* out, long long N,
+                                     int C, int train, float momentum, float eps, void* stream) {
+  if (!z || !gamma || !beta || !stat || !out || !head_ok(N, C) || (train && !sums) ||
+      (!train && (!run_mean || !run_var)) || ((run_mean == nullptr) != (run_var == nullptr)))
+    return ESVIT_ERR_BAD_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  cvt::bn_finalize_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, gamma, beta, run_mean, run_var, nbt, stat, C, train,
+                                                           momentum, eps);
+  const long long n8 = N * C / 8;
+  cvt::bn_normalize_kernel<true><<<cvt::grid_for(n8, 256), 256, 0, st>>>((const bf16*)z, stat, (bf16*)out, C, n8);
+  ESVIT_LAUNCH_CHECK();
+}
+
+ESVIT_API int esvit_headbn_bwd_stats(const void* dy, const void* z, const float* stat, float* part, double* sums,
+                                     float* dgamma, float* dbeta, long long N, int C, void* stream) {
+  if (!dy || !z || !stat || !part || !sums || !head_ok(N, C)) return ESVIT_ERR_BAD_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long nchunk = (N + cvt::PCH - 1) / cvt::PCH;
+  cvt::bn_bwd_partials_kernel<true><<<dim3((unsigned)nchunk, C / 64), cvt::NT, 0, st>>>((const bf16*)dy, (const bf16*)z,
+                                                                                       stat, part, N, C);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return (int)e;
+  return (int)cvt::fold(part, nchunk, 2, C, sums, (double)N, dbeta, dgamma, nullptr, st);
+}
+
+ESVIT_API int esvit_headbn_bwd_apply(const void* dy, const void* z, const float* stat, const double* sums, float* coef,
+                                     void* dz, float* part, float* dbias, long long N, int C, int train, void* stream) {
+  if (!dy || !z || !stat || !coef || !dz || !part || !dbias || (train && !sums) || !head_ok(N, C))
+    return ESVIT_ERR_BAD_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  cvt::bn_bwd_coef_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, stat, coef, C, train);
+  const long long nchunk = (N + cvt::PCH - 1) / cvt::PCH;
+  cvt::head_bwd_dz_kernel<<<dim3((unsigned)nchunk, C / 64), cvt::NT, 0, st>>>((const bf16*)dy, (const bf16*)z, stat, coef,
+                                                                             (bf16*)dz, part, N, C);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return (int)e;
+  return (int)cvt::fold(part, nchunk, 1, C, nullptr, 0.0, dbias, nullptr, nullptr, st);
 }

@@ -333,6 +333,10 @@ def make_step(arch: str = "swin_tiny_w7", out_dim: int = 65536, ncrops: int = 10
     loss = Loss(out_dim, ncrops, teacher_temp, teacher_temp, 0, 100).to(device)
     student_ddp = None
     multi = dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1
+    if multi and (head_kwargs or {}).get("use_bn"):
+        # main_esvit.py:366-373: BN heads -> SyncBatchNorm in both networks (their statistics span every rank's rows)
+        student = nn.SyncBatchNorm.convert_sync_batchnorm(student)
+        teacher = nn.SyncBatchNorm.convert_sync_batchnorm(teacher)
     if ddp and multi and optimizer != "fused":
         student_ddp = nn.parallel.DistributedDataParallel(student, device_ids=[torch.cuda.current_device()])
     if optimizer == "fused":

@@ -66,6 +66,18 @@ class LinearFn(Function):
         return dx, dw, None, None
 
 
+class LinearColsumFn(LinearFn):
+    """LinearFn whose bias gradient is the column sums of dy (ops.colsum), for a Linear whose consumer kernel does not
+    produce it: the last Linear of DINOHead(use_bn=True), read by the row L2 normalisation."""
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        dx, dw, _, _ = LinearFn.backward(ctx, g)
+        db = ops.colsum(g.reshape(-1, g.shape[-1]).contiguous()) if ctx.needs_input_grad[3] else None
+        return dx, dw, None, db
+
+
 class MlpFn(Function):
     """fc2(gelu(fc1(x))) (models/swin_transformer.py:31-35).  forward at C in ops.MLP_FUSED_C (Swin stages 0-1): ONE
     back-to-back kernel (esvit_mlp_fwd) writes y and, when a gradient is needed, h and gelu'; at other C: h, gelu' from ONE

@@ -1225,6 +1225,66 @@ class DwBnFn(Function):
                 None, None, None, None)
 
 
+class HeadBnGeluFn(Function):
+    """One Linear -> BatchNorm1d -> GELU unit of DINOHead(use_bn=True) (models/vision_transformer.py:389-397), called once
+    on the rows of every crop: z = x . w16^T + bias (bias-epilogue GEMM, bf16 [R, C]), then gelu(BN(z)) bf16 [R, C] for
+    the next GEMM.  `bn` (BatchNorm1d or SyncBatchNorm) holds gamma / beta and the running buffers; train: the batch
+    statistics of z (fp64 column sums, esvit_headbn_fwd_stats), the running statistics updated in place; else the running
+    statistics.  pg: the process group of a SyncBatchNorm (world size > 1) or None; the column sums (and the count) are
+    then all-reduced, forward and backward, as in DwBnFn.  backward: the BN input gradient through GELU' (bf16), the bias
+    / gamma / beta gradients from the BN kernels (local sums: DDP averages them), dx and the fp32 dW from the GEMM family."""
+
+    @staticmethod
+    def forward(ctx, x, wp, w16, bias, gamma, beta, bn, train: bool, pg):
+        x = _chk(x, BF16, "x")
+        gamma, beta = _chk(gamma, F32, "gamma"), _chk(beta, F32, "beta")
+        R, C = x.shape[0], w16.shape[0]
+        if train and pg is None and R == 1:
+            raise ValueError(f"Expected more than 1 value per channel when training, got input size {(R, C)}")
+        z = gemm(x, w16, bias)
+        out = torch.empty_like(z)
+        stat = torch.empty(4 * C, dtype=F32, device=x.device)
+        sums = None
+        if train:
+            part = torch.empty(-(-R // 256) * 2 * C, dtype=F32, device=x.device)
+            sums = torch.empty(2 * C + 1, dtype=torch.float64, device=x.device)
+            _lib.call("esvit_headbn_fwd_stats", _p(z), _p(part), _p(sums), R, C, _stream())
+            if pg is not None:
+                torch.distributed.all_reduce(sums, group=pg)
+        rm, rv, nbt = bn.running_mean, bn.running_var, bn.num_batches_tracked
+        _lib.call("esvit_headbn_fwd_apply", _p(z), _p(gamma), _p(beta), _p(sums), _p(rm), _p(rv),
+                  _p(nbt) if (train and nbt is not None) else None, _p(stat), _p(out), R, C, 1 if train else 0,
+                  float(bn.momentum) if bn.momentum is not None else 0.0, float(bn.eps), _stream())
+        ctx.save_for_backward(x, w16, z, stat)
+        ctx.meta = (train, pg, tuple(wp.shape), gamma.data_ptr(), bias.data_ptr())
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        x, w16, z, stat = ctx.saved_tensors
+        train, pg, wshape, gptr, bptr = ctx.meta
+        g = _chk(g, BF16, "g")
+        R, C = z.shape
+        dev = z.device
+        part = torch.empty(-(-R // 256) * 2 * C, dtype=F32, device=dev)
+        bsums = torch.empty(2 * C + 1, dtype=torch.float64, device=dev)
+        coef = torch.empty(3 * C, dtype=F32, device=dev)
+        aff, first_a = _acc(("bn", gptr), (2, C), dev)  # dgamma | dbeta
+        db, first_b = _acc(("bias", bptr), (C,), dev)
+        _lib.call("esvit_headbn_bwd_stats", _p(g), _p(z), _p(stat), _p(part), _p(bsums), _p(aff[0]), _p(aff[1]), R, C,
+                  _stream())
+        if train and pg is not None:
+            torch.distributed.all_reduce(bsums, group=pg)
+        dz = torch.empty_like(z)
+        _lib.call("esvit_headbn_bwd_apply", _p(g), _p(z), _p(stat), _p(bsums), _p(coef), _p(dz), _p(part), _p(db), R, C,
+                  1 if train else 0, _stream())
+        dw = gemm_wgrad(dz, x).view(wshape) if ctx.needs_input_grad[1] else None
+        dx = gemm(dz, w16, None, b_mn=True) if ctx.needs_input_grad[0] else None
+        return (dx, dw, None, db if first_b else None, aff[0] if first_a else None, aff[1] if first_a else None,
+                None, None, None)
+
+
 class MhsaWinGroupsFn(Function):
     """Window attention of CvT (Attention.forward :180-218; no mask, no bias) at head dim 64: qkv bf16 [Tp, 3C] of the
     padded maps (pw GEMM output incl. bias) -> the cropped output bf16 [T, C]; groups as DwBnFn's.  One launch per group.

@@ -11,6 +11,8 @@ csrc/vit_embed.cu.
 
 DINOHead (:384-418): mlp.{0,2,4} Linear(+exact GELU) -> L2 normalise -> weight-normed Linear(bottleneck, out_dim,
 bias=False), with parameters ``mlp.N.{weight,bias}``, ``last_layer.weight_g`` [K,1], ``last_layer.weight_v`` [K,D].
+With use_bn=True each hidden Linear is followed by a real nn.BatchNorm1d (``mlp.{1,4}.*``; so utils.has_batchnorms and
+nn.SyncBatchNorm.convert_sync_batchnorm work unchanged) and the MLP runs as ops.HeadBnGeluFn units.
 The three MLP GEMMs and the last-layer GEMM are bf16 library GEMMs; GELU, the row normalisation and the
 weight-norm reparameterisation (fwd + bwd) are esvit_b200 kernels.  Output logits are bf16 [rows, out_dim]
 (what the reference produces under autocast); the losses consume them without an fp32 copy.
@@ -24,9 +26,11 @@ from typing import List, Optional, Sequence, Tuple
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+from torch.nn.modules.batchnorm import _BatchNorm
 
 from . import backbone, linear, ops, shadow
 from .backbone import MultiCropBackbone, _CastCache
+from .cvt_v4_transformer import _sync_group
 from .swin_transformer import USE_GEMM2, Mlp, _lin_c
 
 Tensor = torch.Tensor
@@ -58,15 +62,15 @@ class DINOHead(nn.Module):
     def __init__(self, in_dim, out_dim, use_bn=False, norm_last_layer=True, nlayers=3, hidden_dim=2048,
                  bottleneck_dim=256):
         super().__init__()
-        if use_bn:
-            raise NotImplementedError("use_bn_in_head is False in every EsViT recipe")
         nlayers = max(nlayers, 1)
         if nlayers == 1:
             self.mlp = nn.Linear(in_dim, bottleneck_dim)
         else:
-            layers = [nn.Linear(in_dim, hidden_dim), nn.GELU()]
+            bn = [nn.BatchNorm1d(hidden_dim)] if use_bn else []
+            layers = [nn.Linear(in_dim, hidden_dim)] + bn + [nn.GELU()]
             for _ in range(nlayers - 2):
-                layers += [nn.Linear(hidden_dim, hidden_dim), nn.GELU()]
+                bn = [nn.BatchNorm1d(hidden_dim)] if use_bn else []
+                layers += [nn.Linear(hidden_dim, hidden_dim)] + bn + [nn.GELU()]
             layers.append(nn.Linear(hidden_dim, bottleneck_dim))
             self.mlp = nn.Sequential(*layers)
         self.apply(self._init_weights)
@@ -84,6 +88,8 @@ class DINOHead(nn.Module):
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         x = x.to(BF16)
         mods = [self.mlp] if isinstance(self.mlp, nn.Linear) else list(self.mlp)
+        if any(isinstance(m, _BatchNorm) for m in mods):
+            return self.last_layer(ops.L2NormFn.apply(self._mlp_bn(x, mods), 1e-12))
         lins = [m for m in mods if isinstance(m, nn.Linear)]
         if USE_GEMM2 and len(lins) == 3 and len(mods) == 5:
             args = []
@@ -103,6 +109,26 @@ class DINOHead(nn.Module):
                     x = F.linear(x, shadow.as_bf16(m.weight), shadow.as_bf16(m.bias))
         x = ops.L2NormFn.apply(x, 1e-12)
         return self.last_layer(x)
+
+    @staticmethod
+    def _mlp_bn(x: Tensor, mods) -> Tensor:
+        """the use_bn MLP: each Linear -> BatchNorm1d / SyncBatchNorm -> GELU is one ops.HeadBnGeluFn; the BN module's
+        mode decides (train: batch statistics over all rows, running statistics updated; eval: running statistics)."""
+        i = 0
+        while i < len(mods):
+            lin = mods[i]
+            w16 = shadow.as_bf16(lin.weight, track_grad=False)
+            if i + 1 < len(mods) and isinstance(mods[i + 1], _BatchNorm):
+                bn = mods[i + 1]
+                train = bn.training or not bn.track_running_stats
+                if train and bn.track_running_stats and bn.momentum is None:
+                    raise NotImplementedError("BatchNorm1d(momentum=None) (cumulative running average) is not implemented")
+                x = ops.HeadBnGeluFn.apply(x, lin.weight, w16, lin.bias, bn.weight, bn.bias, bn, train, _sync_group(bn))
+                i += 3  # Linear, BN, GELU
+            else:
+                x = linear.LinearColsumFn.apply(x, lin.weight, w16, lin.bias)
+                i += 1
+        return x
 
 
 # ---------------------------------------------------------------------------------------------------------------------

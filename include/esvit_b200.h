@@ -254,6 +254,23 @@ int esvit_dwbn_bwd_apply(const void* dy, const void* z, const void* y, const flo
                          const double* sums, float* coef, void* dx, float* part, float* dw, int B, int H, int W, int Hp,
                          int Wp, int C, int train, void* stream);
 
+/* ---- DINOHead(use_bn=True) (models/vision_transformer.py:389-397): Linear -> BatchNorm1d -> exact GELU ------------------
+ * z bf16 [N, C] is the bias-GEMM output, C % 64 == 0.  The statistics, running-statistics and coefficient arithmetic is
+ * the dwbn_* one.  fwd_stats: sums fp64 [2C + 1] = (sum z, sum z^2, count N).  fwd_apply: stat fp32 [4C] as dwbn_fwd_apply
+ * (train: run_mean / run_var / nbt updated in place when given; train = 0: the running statistics), out bf16 [N, C] =
+ * gelu(z * stat[2] + stat[3]).  bwd_stats: with dh = dy gelu'(z * stat[2] + stat[3]), sums fp64 [2C + 1] = (sum dh,
+ * sum dh xhat, count); dbeta / dgamma fp32 [C] += the local sums.  bwd_apply: dz bf16 [N, C] (written) = the BN input
+ * gradient, dbias fp32 [C] += column sums of dz; coef fp32 [3C] scratch.  part: fp32 scratch of ceil(N / 256) * 2 * C
+ * floats.  A SyncBatchNorm all-reduces `sums` between *_stats and *_apply.  No floating-point atomics. */
+int esvit_headbn_fwd_stats(const void* z, float* part, double* sums, long long N, int C, void* stream);
+int esvit_headbn_fwd_apply(const void* z, const float* gamma, const float* beta, const double* sums, float* run_mean,
+                           float* run_var, long long* nbt, float* stat, void* out, long long N, int C, int train,
+                           float momentum, float eps, void* stream);
+int esvit_headbn_bwd_stats(const void* dy, const void* z, const float* stat, float* part, double* sums, float* dgamma,
+                           float* dbeta, long long N, int C, void* stream);
+int esvit_headbn_bwd_apply(const void* dy, const void* z, const float* stat, const double* sums, float* coef, void* dz,
+                           float* part, float* dbias, long long N, int C, int train, void* stream);
+
 /* ---- Vision Longformer (layers/longformer2d.py Long2DSCSelfAttention, W = 7, one global token, head dim 32) --------
  * Per image N = 1 + nx*ny token rows, row 0 the global token: q bf16 [B*N, C] (unscaled), kv bf16 [B*N, 2C] as [k|v],
  * out / dout / dq bf16 [B*N, C], dkv bf16 [B*N, 2C]; C = 32 nH.  mode int32 [1] in device memory: 0 = all nine
