@@ -1,18 +1,19 @@
-"""CvT-13 pre-training step on one GPU: spec s1, 2 x 224^2 + 8 x 96^2 crops, DDINOLoss (dense), K = 65 536.
+"""CvT-13 pre-training step on one GPU: spec s1 (--arch cvt_13, windows 7) or win_size/s1 (--arch cvt_13_w14, windows
+14, 14, 14, 7), 2 x 224^2 + 8 x 96^2 crops, DDINOLoss (dense), K = 65 536.
 
-    python bench_cvt.py [--batch 64] [--steps 10] [--warmup 3] [--no-reference]
+    python bench_cvt.py [--arch cvt_13] [--batch 64] [--steps 10] [--warmup 3] [--no-reference]
 
 Prints one JSON line:
-  * `value`: images/s of esvit_b200's captured step (engine.make_step("cvt_13"), CUDA graph, loss read back every step
+  * `value`: images/s of esvit_b200's captured step (engine.make_step(arch), CUDA graph, loss read back every step
     as train_one_epoch does) at the largest batch of --batch, 48, 32, 16 that fits, reported as `batch`;
-  * `reference`: the UNMODIFIED reference modules (models.cvt_v4_transformer.CvT built as get_cls_model builds it,
-    DINOHead, DDINOLoss from oracle/_ref/, installed by build()) through main_esvit.py:541-590's statement sequence under
-    bf16 autocast, student and teacher in train mode, at the largest batch that fits; "not run" with the reason when
-    the tree is absent or nothing fits;
+  * `reference`: the UNMODIFIED reference modules (models.cvt_v4_transformer.CvT built as get_cls_model builds it from
+    the arch's MODEL.SPEC, DINOHead, DDINOLoss from oracle/_ref/, installed by build()) through main_esvit.py:541-590's
+    statement sequence under bf16 autocast, student and teacher in train mode, at the largest batch that fits; "not
+    run" with the reason when the tree is absent or nothing fits;
   * `kernels`: CUDA-event times per step of the CvT kernels (conv-embed gather / col2im, depthwise + BN forward /
     backward, window attention forward / backward) with their algorithmic bytes (and FLOPs for attention), achieved
     TB/s, and share of the bound the data sheet gives (the larger of FLOPs / 989 TFLOP/s and bytes / 3.35 TB/s), from
-    an eager step;
+    an eager step; for cvt_13_w14 also `attention_by_L`, the window attention split by tokens per window L = w^2;
   * `gpu`: card name, power limit and maximum SM clock, read in the same run.
 Nothing is written to the tree.
 """
@@ -91,34 +92,47 @@ def _cost(r) -> tuple:
     return Tp * 3 * r["C"] * 2 * 2 + T * r["C"] * 2 * 2 + Tp * r["nH"] * 8, 2.5 * flops
 
 
+def _rates(rows) -> dict:
+    ms = sum(r["ms"] for r in rows)
+    nbytes = sum(_cost(r)[0] for r in rows)
+    flops = sum(_cost(r)[1] for r in rows)
+    bound_ms = max(flops / (PEAK_TFLOPS * 1e12), nbytes / (PEAK_TBS * 1e12)) * 1e3
+    return {"ms_per_step": round(ms, 3), "launches": len(rows), "gb": round(nbytes / 1e9, 3),
+            "tb_s": round(nbytes / ms / 1e9, 3), "tflops": round(flops / ms / 1e9, 1),
+            "share_of_bound": round(bound_ms / ms, 3),
+            "bound": "tensor" if flops / PEAK_TFLOPS > nbytes / PEAK_TBS else "hbm"}
+
+
+def _attention_by_L(res) -> dict:
+    """window attention forward / backward per window size: {"L=196": {"fwd": rates, "bwd": rates}, ...}"""
+    out = {}
+    for L in sorted({r["w"] * r["w"] for r in res if r["name"].startswith("esvit_mhsa_win")}, reverse=True):
+        out[f"L={L}"] = {d: _rates([r for r in res if r["name"] == f"esvit_mhsa_win_{d}" and r["w"] * r["w"] == L])
+                         for d in ("fwd", "bwd")}
+    return out
+
+
 def _kernel_rates(res) -> dict:
     out = {}
     for name in NAMES:
         rows = [r for r in res if r["name"] == name]
         if not rows:
             continue
-        ms = sum(r["ms"] for r in rows)
-        nbytes = sum(_cost(r)[0] for r in rows)
-        flops = sum(_cost(r)[1] for r in rows)
-        bound_ms = max(flops / (PEAK_TFLOPS * 1e12), nbytes / (PEAK_TBS * 1e12)) * 1e3
-        out[name] = {"ms_per_step": round(ms, 3), "launches": len(rows), "gb": round(nbytes / 1e9, 3),
-                     "tb_s": round(nbytes / ms / 1e9, 3), "tflops": round(flops / ms / 1e9, 1),
-                     "share_of_bound": round(bound_ms / ms, 3),
-                     "bound": "tensor" if flops / PEAK_TFLOPS > nbytes / PEAK_TBS else "hbm"}
+        out[name] = _rates(rows)
     return out
 
 
-def run_ours(B: int, steps: int, warmup: int) -> dict:
+def run_ours(arch: str, B: int, steps: int, warmup: int) -> dict:
     from esvit_b200 import _lib, engine
-    step, student, teacher, loss = engine.make_step(arch="cvt_13", out_dim=K, ncrops=NCROPS, dense=True,
-                                                    cuda_graph=True)
+    step, student, teacher, loss = engine.make_step(arch=arch, out_dim=K, ncrops=NCROPS, dense=True, cuda_graph=True)
     imgs = crops(B)
     float(step(imgs, 1, LR, WD, MOM))                    # eager warm-up 1 (module loads, allocator)
     _lib.reset_counters()
     _lib.time_entry_point(list(NAMES))
     float(step(imgs, 1, LR, WD, MOM))                    # eager warm-up 2, timed per launch
     torch.cuda.synchronize()
-    kernels = _kernel_rates(_lib.timed_results())
+    timed = _lib.timed_results()
+    kernels = _kernel_rates(timed)
     _lib.time_entry_point(None)
     for _ in range(warmup):                              # warm-up 3, then capture + replays
         float(step(imgs, 1, LR, WD, MOM))
@@ -129,6 +143,8 @@ def run_ours(B: int, steps: int, warmup: int) -> dict:
     ms = _timed(one, steps)
     res = {"ms_per_step": round(ms, 2), "images_per_s": round(B / ms * 1e3, 1), "last_loss": last[0],
            "peak_mem_gib": round(torch.cuda.max_memory_allocated() / 2 ** 30, 1), "kernels": kernels}
+    if arch != "cvt_13":
+        res["attention_by_L"] = _attention_by_L(timed)
     del step, student, teacher, loss
     return res
 
@@ -137,7 +153,7 @@ class _ReferenceStep:
     """main_esvit.py:280-301 (CvT student / teacher with DINOHeads) and :541-590 (autocast bf16 forward + loss,
     loss.item(), backward, clip_gradients, cancel_gradients_last_layer, AdamW step, EMA) on the unmodified modules."""
 
-    def __init__(self):
+    def __init__(self, spec: dict):
         from oracle import reference_import as RI
         import torch.distributed as dist
         ns = RI.load()
@@ -149,13 +165,12 @@ class _ReferenceStep:
                 os.environ.setdefault("MASTER_PORT", str(sk.getsockname()[1]))
             dist.init_process_group("nccl", rank=0, world_size=1, device_id=torch.device("cuda", torch.cuda.current_device()))
         from models import cvt_v4_transformer as ref_cvt
-        from esvit_b200.cvt_v4_transformer import S1_SPEC
         from functools import partial
         torch.manual_seed(0)
 
         def build(dpr):   # get_cls_model (:685-707) without the yacs config
             return ref_cvt.CvT(num_classes=0, act_layer=ref_cvt.QuickGELU, norm_layer=partial(ref_cvt.LayerNorm, eps=1e-5),
-                               init="trunc_norm", use_dense_prediction=True, spec=dict(S1_SPEC, DROP_PATH_RATE=dpr))
+                               init="trunc_norm", use_dense_prediction=True, spec=dict(spec, DROP_PATH_RATE=dpr))
         self.student, self.teacher = build(0.1), build(0.0)
         for m in (self.student, self.teacher):   # main_esvit.py never calls .eval(): BatchNorm in train mode
             m.head = ns.DINOHead(768, K)
@@ -192,8 +207,9 @@ class _ReferenceStep:
         return lv
 
 
-def run_reference(B: int, steps: int, warmup: int) -> dict:
-    ref = _ReferenceStep()
+def run_reference(arch: str, B: int, steps: int, warmup: int) -> dict:
+    from esvit_b200.engine import CVT_SPECS
+    ref = _ReferenceStep(CVT_SPECS[arch]["cvt_spec"])
     imgs = crops(B)
     for _ in range(warmup):
         ref.step(imgs)
@@ -214,6 +230,7 @@ def largest_fitting(fn, batches):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--arch", choices=("cvt_13", "cvt_13_w14"), default="cvt_13")
     ap.add_argument("--batch", type=int, default=64)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
@@ -223,7 +240,7 @@ def main():
         sys.exit("bench_cvt.py measures on a CUDA device; none found")
     from oracle import reference_import as RI
     batches = [b for b in (args.batch, 48, 32, 16) if b <= args.batch]
-    B, ours = largest_fitting(lambda b: run_ours(b, args.steps, args.warmup), batches)
+    B, ours = largest_fitting(lambda b: run_ours(args.arch, b, args.steps, args.warmup), batches)
     torch.cuda.empty_cache()
     torch.cuda.reset_peak_memory_stats()
     if args.no_reference:
@@ -231,9 +248,10 @@ def main():
     elif not RI.available():
         ref = "not run (reference tree not installed under oracle/_ref/)"
     else:
-        rb, r = largest_fitting(lambda b: run_reference(b, args.steps, args.warmup), batches)
+        rb, r = largest_fitting(lambda b: run_reference(args.arch, b, args.steps, args.warmup), batches)
         ref = dict(r, batch=rb) if rb is not None else f"not run ({r})"
-    line = {"metric": "multi-crop images/sec, CvT-13 (s1) pretrain step (2 global 224^2 + 8 local 96^2 crops, "
+    spec = "s1" if args.arch == "cvt_13" else "win_size/s1"
+    line = {"metric": f"multi-crop images/sec, CvT-13 ({spec}) pretrain step (2 global 224^2 + 8 local 96^2 crops, "
                       "DDINOLoss, K=65536)",
             "value": ours["images_per_s"] if B else None, "unit": "images/s", "batch": B,
             "steps": args.steps, "warmup": args.warmup, "ours": ours, "reference": ref, "gpu": gpu_info()}

@@ -18,10 +18,13 @@
 // Each output row is owned by exactly one warp.
 //
 // Window mode (WIN = true; CvT, models/cvt_v4_transformer.py Attention.forward :165-220): "sequence" s is window s of
-// the zero-padded Hp x Wp token map (images, then windows row-major, then tokens row-major), L = w*w <= 64 tokens.  q / k
+// the zero-padded Hp x Wp token map (images, then windows row-major, then tokens row-major), L = w*w tokens (any w; the
+// 64-row query / key tiles loop as in the dense mode, window token r0 + r in row r of the tile that starts at r0).  q / k
 // / v rows are gathered from the token-major qkv [B*Hp*Wp, 3C] of the padded map; out / dout are the CROPPED map
 // [B*H*W, C]: padded query rows are not stored (their dO reads as 0, so their dq is 0), padded keys take part as in the
 // reference.  lse / dvec are [windows, nH, L] as in the dense mode.
+#include <climits>
+
 #include "wa_common.cuh"
 
 namespace mh {
@@ -125,17 +128,17 @@ __device__ __forceinline__ long long win_out_row(const Win& g, int s, int l) {
   return (y < g.H && x < g.W) ? ((long long)img * g.H + y) * g.W + x : -1;
 }
 
-// load_tile for the rows of window s: src = row 0's column base, row r at (out ? cropped : padded) row of token r;
-// rows >= L and padded rows of the cropped map are zero
+// load_tile for tokens r0.. of window s: src = the map's column base, tile row r at the (out ? cropped : padded) row of
+// token r0 + r; tokens >= L and padded rows of the cropped map are zero
 template <bool OUT>
 __device__ __forceinline__ void load_tile_win(bf16* dst, const bf16* __restrict__ src, long long ld, const Win& g, int s,
-                                              int L) {
+                                              int L, int r0) {
 #pragma unroll
   for (int k = 0; k < 4; k++) {
     const int e = threadIdx.x + k * NTHR;
     const int r = e >> 3, c = (e & 7) * 8;
     long long row = -1;
-    if (r < L) row = OUT ? win_out_row(g, s, r) : win_row(g, s, r);
+    if (r0 + r < L) row = OUT ? win_out_row(g, s, r0 + r) : win_row(g, s, r0 + r);
     const bool ok = row >= 0;
     cp_async16(dst + r * LDS + c, src + (ok ? row * ld : 0) + c, ok ? 16 : 0);
   }
@@ -177,16 +180,16 @@ __global__ void __launch_bounds__(NTHR) mhsa_fwd_kernel(const bf16* __restrict__
   const long long C3 = 3LL * C;
   const bf16* base = qkv + (long long)b * L * C3 + h * HD;
   if constexpr (WIN) {
-    load_tile_win<false>(Qs, qkv + h * HD, C3, win, b, L);
-    load_tile_win<false>(Qs + TILE, qkv + h * HD + C, C3, win, b, L);
-    load_tile_win<false>(Qs + 2 * TILE, qkv + h * HD + 2 * C, C3, win, b, L);
+    load_tile_win<false>(Qs, qkv + h * HD, C3, win, b, L, q0);
+    load_tile_win<false>(Qs + TILE, qkv + h * HD + C, C3, win, b, L, 0);
+    load_tile_win<false>(Qs + 2 * TILE, qkv + h * HD + 2 * C, C3, win, b, L, 0);
   } else {
     load_tile(Qs, base + q0 * C3, C3, L - q0);
     load_tile(Qs + TILE, base + C, C3, L);
     load_tile(Qs + 2 * TILE, base + 2 * C, C3, L);
   }
   cp_async_commit();
-  const int nkt = WIN ? 1 : (L + 63) / 64;
+  const int nkt = (L + 63) / 64;
   float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
   float o[8][4];
 #pragma unroll
@@ -196,8 +199,13 @@ __global__ void __launch_bounds__(NTHR) mhsa_fwd_kernel(const bf16* __restrict__
     const int st = kt & 1;
     if (kt + 1 < nkt) {
       bf16* nx = Qs + (1 + 2 * (st ^ 1)) * TILE;
-      load_tile(nx, base + C + (kt + 1) * 64 * C3, C3, L - (kt + 1) * 64);
-      load_tile(nx + TILE, base + 2 * C + (kt + 1) * 64 * C3, C3, L - (kt + 1) * 64);
+      if constexpr (WIN) {
+        load_tile_win<false>(nx, qkv + h * HD + C, C3, win, b, L, (kt + 1) * 64);
+        load_tile_win<false>(nx + TILE, qkv + h * HD + 2 * C, C3, win, b, L, (kt + 1) * 64);
+      } else {
+        load_tile(nx, base + C + (kt + 1) * 64 * C3, C3, L - (kt + 1) * 64);
+        load_tile(nx + TILE, base + 2 * C + (kt + 1) * 64 * C3, C3, L - (kt + 1) * 64);
+      }
     }
     cp_async_commit();
     cp_async_wait<1>();
@@ -302,10 +310,10 @@ __global__ void __launch_bounds__(NTHR) mhsa_bwd_dq_kernel(const bf16* __restric
   const long long C3 = 3LL * C;
   const bf16* base = qkv + (long long)b * L * C3 + h * HD;
   if constexpr (WIN) {
-    load_tile_win<false>(Qs, qkv + h * HD, C3, win, b, L);
-    load_tile_win<true>(Qs + TILE, dout + h * HD, C, win, b, L);
-    load_tile_win<false>(Qs + 2 * TILE, qkv + h * HD + C, C3, win, b, L);
-    load_tile_win<false>(Qs + 3 * TILE, qkv + h * HD + 2 * C, C3, win, b, L);
+    load_tile_win<false>(Qs, qkv + h * HD, C3, win, b, L, q0);
+    load_tile_win<true>(Qs + TILE, dout + h * HD, C, win, b, L, q0);
+    load_tile_win<false>(Qs + 2 * TILE, qkv + h * HD + C, C3, win, b, L, 0);
+    load_tile_win<false>(Qs + 3 * TILE, qkv + h * HD + 2 * C, C3, win, b, L, 0);
   } else {
     load_tile(Qs, base + q0 * C3, C3, L - q0);
     load_tile(Qs + TILE, dout + ((long long)b * L + q0) * C + h * HD, C, L - q0);
@@ -318,7 +326,7 @@ __global__ void __launch_bounds__(NTHR) mhsa_bwd_dq_kernel(const bf16* __restric
   const float* dp = dvec + ((long long)b * nH + h) * L;
   const float lA = rA < L ? lp[rA] * LOG2E : 0.f, lB = rB < L ? lp[rB] * LOG2E : 0.f;
   const float DA = rA < L ? dp[rA] : 0.f, DB = rB < L ? dp[rB] : 0.f;
-  const int nkt = WIN ? 1 : (L + 63) / 64;
+  const int nkt = (L + 63) / 64;
   float dq[8][4];
 #pragma unroll
   for (int dt = 0; dt < 8; dt++) dq[dt][0] = dq[dt][1] = dq[dt][2] = dq[dt][3] = 0.f;
@@ -327,8 +335,13 @@ __global__ void __launch_bounds__(NTHR) mhsa_bwd_dq_kernel(const bf16* __restric
     const int st = kt & 1;
     if (kt + 1 < nkt) {
       bf16* nx = Qs + (2 + 2 * (st ^ 1)) * TILE;
-      load_tile(nx, base + C + (kt + 1) * 64 * C3, C3, L - (kt + 1) * 64);
-      load_tile(nx + TILE, base + 2 * C + (kt + 1) * 64 * C3, C3, L - (kt + 1) * 64);
+      if constexpr (WIN) {
+        load_tile_win<false>(nx, qkv + h * HD + C, C3, win, b, L, (kt + 1) * 64);
+        load_tile_win<false>(nx + TILE, qkv + h * HD + 2 * C, C3, win, b, L, (kt + 1) * 64);
+      } else {
+        load_tile(nx, base + C + (kt + 1) * 64 * C3, C3, L - (kt + 1) * 64);
+        load_tile(nx + TILE, base + 2 * C + (kt + 1) * 64 * C3, C3, L - (kt + 1) * 64);
+      }
     }
     cp_async_commit();
     cp_async_wait<1>();
@@ -369,11 +382,12 @@ __global__ void __launch_bounds__(NTHR) mhsa_bwd_dq_kernel(const bf16* __restric
 }
 
 // dK, dV of 64 key rows
+// (WIN: at most 168 registers, so three CTAs fit an SM as they did when a window was a single tile)
 template <bool WIN>
-__global__ void __launch_bounds__(NTHR) mhsa_bwd_dkdv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
-                                                             const float* __restrict__ lse, const float* __restrict__ dvec,
-                                                             bf16* __restrict__ dqkv, int L, int C, int nH, float c2,
-                                                             float scale, const Win win) {
+__global__ void __launch_bounds__(NTHR, WIN ? 3 : 0)
+    mhsa_bwd_dkdv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, const float* __restrict__ lse,
+                         const float* __restrict__ dvec, bf16* __restrict__ dqkv, int L, int C, int nH, float c2,
+                         float scale, const Win win) {
   extern __shared__ __align__(16) unsigned char smraw[];
   bf16* Ks = reinterpret_cast<bf16*>(smraw);            // [K | V | Q0 | dO0 | Q1 | dO1]
   float* stat = reinterpret_cast<float*>(Ks + 6 * TILE);  // [2 stages][lse' 64 | D 64]
@@ -385,10 +399,10 @@ __global__ void __launch_bounds__(NTHR) mhsa_bwd_dkdv_kernel(const bf16* __restr
   const float* lp = lse + ((long long)b * nH + h) * L;
   const float* dp = dvec + ((long long)b * nH + h) * L;
   if constexpr (WIN) {
-    load_tile_win<false>(Ks, qkv + h * HD + C, C3, win, b, L);
-    load_tile_win<false>(Ks + TILE, qkv + h * HD + 2 * C, C3, win, b, L);
-    load_tile_win<false>(Ks + 2 * TILE, qkv + h * HD, C3, win, b, L);
-    load_tile_win<true>(Ks + 3 * TILE, dout + h * HD, C, win, b, L);
+    load_tile_win<false>(Ks, qkv + h * HD + C, C3, win, b, L, k0);
+    load_tile_win<false>(Ks + TILE, qkv + h * HD + 2 * C, C3, win, b, L, k0);
+    load_tile_win<false>(Ks + 2 * TILE, qkv + h * HD, C3, win, b, L, 0);
+    load_tile_win<true>(Ks + 3 * TILE, dout + h * HD, C, win, b, L, 0);
   } else {
     load_tile(Ks, base + C + k0 * C3, C3, L - k0);
     load_tile(Ks + TILE, base + 2 * C + k0 * C3, C3, L - k0);
@@ -401,7 +415,7 @@ __global__ void __launch_bounds__(NTHR) mhsa_bwd_dkdv_kernel(const bf16* __restr
     stat[q] = q < L ? lp[q] * LOG2E : INFINITY;
     stat[64 + q] = q < L ? dp[q] : 0.f;
   }
-  const int nqt = WIN ? 1 : (L + 63) / 64;
+  const int nqt = (L + 63) / 64;
   float dk[8][4], dv[8][4];
 #pragma unroll
   for (int dt = 0; dt < 8; dt++)
@@ -413,8 +427,13 @@ __global__ void __launch_bounds__(NTHR) mhsa_bwd_dkdv_kernel(const bf16* __restr
     if (qt + 1 < nqt) {
       bf16* nx = Ks + (2 + 2 * (st ^ 1)) * TILE;
       const int n0 = (qt + 1) * 64;
-      load_tile(nx, base + n0 * C3, C3, L - n0);
-      load_tile(nx + TILE, gbase + (long long)n0 * C, C, L - n0);
+      if constexpr (WIN) {
+        load_tile_win<false>(nx, qkv + h * HD, C3, win, b, L, n0);
+        load_tile_win<true>(nx + TILE, dout + h * HD, C, win, b, L, n0);
+      } else {
+        load_tile(nx, base + n0 * C3, C3, L - n0);
+        load_tile(nx + TILE, gbase + (long long)n0 * C, C, L - n0);
+      }
       if (threadIdx.x < 64) {
         const int q = n0 + threadIdx.x;
         float* sn = stat + (st ^ 1) * 128;
@@ -483,14 +502,15 @@ static cudaError_t opt_in(K kernel, size_t smem) {
                           : cudaSuccess;
 }
 
-// window geometry of a B x H x W map in windows of w x w (rejects what the WIN kernels cannot address)
+// window geometry of a B x H x W map in windows of w x w (rejects what the WIN kernels cannot address: the window
+// count is a grid dimension, and the token rows of the padded map are counted in int by the prep grid)
 static bool win_geo(int B, int H, int W, int w, Win* g, int* nwin_total) {
-  if (B < 1 || H < 1 || W < 1 || w < 1 || w * w > 64 || w > H || w > W) return false;
+  if (B < 1 || H < 1 || W < 1 || w < 1 || w > H || w > W) return false;
   g->H = H; g->W = W; g->w = w;
   g->Hp = (H + w - 1) / w * w; g->Wp = (W + w - 1) / w * w;
   g->nwx = g->Wp / w; g->nwin = (g->Hp / w) * g->nwx;
   const long long n = (long long)B * g->nwin;
-  if (n > 65535) return false;
+  if (n > 65535 || n * w * w > INT_MAX) return false;
   *nwin_total = (int)n;
   return true;
 }

@@ -1,5 +1,5 @@
-"""CvT backbone (models/cvt_v4_transformer.py, spec experiments/imagenet/cvt_v4/s1.yaml) behind the reference's
-signatures and state_dict keys.
+"""CvT backbone (models/cvt_v4_transformer.py, specs experiments/imagenet/cvt_v4/s1.yaml and win_size/s1.yaml) behind
+the reference's signatures and state_dict keys.
 
 CvT / get_cls_model take the reference's MODEL.SPEC keys and hold the reference's parameters AND buffers
 (``stage{i}.0.{proj,norm}.*``, ``stage{i}.1.layers.{j}.0.{norm,fn.qkv.dw,fn.qkv.bn,fn.qkv.pw,fn.proj_out}.*``,
@@ -186,11 +186,11 @@ class CvT(MultiCropBackbone):
         super().__init__()
         self.num_stages = spec['NUM_STAGES']
         if spec['REL_POS_EMBED']:
-            raise NotImplementedError("CvT: REL_POS_EMBED is not implemented (spec s1 only)")
+            raise NotImplementedError("CvT: REL_POS_EMBED is not implemented")
         if any(spec['SHIFT'][:self.num_stages]):
-            raise NotImplementedError("CvT: shifted windows are not implemented (spec s1 only)")
+            raise NotImplementedError("CvT: shifted windows are not implemented")
         if _spec(spec, 'RES_STEM', False):
-            raise NotImplementedError("CvT: RES_STEM is not implemented (spec s1 only)")
+            raise NotImplementedError("CvT: RES_STEM is not implemented")
         if act_layer is not QuickGELU:
             raise NotImplementedError("CvT: the FeedForward activation is QuickGELU (get_cls_model)")
         for i in range(self.num_stages):
@@ -199,8 +199,8 @@ class CvT(MultiCropBackbone):
                 raise NotImplementedError(f"CvT: head dim 64 only (stage {i}: dim {dim}, {heads} heads)")
             if spec['KERNEL_QKV'][i] != 3 or spec['PADDING_QKV'][i] != 1:
                 raise NotImplementedError("CvT: KERNEL_QKV 3 with PADDING_QKV 1 only")
-            if not 1 <= spec['WINDOW_SIZE'][i] <= 8:
-                raise NotImplementedError("CvT: window sizes 1..8 only (w * w <= 64)")
+            if spec['WINDOW_SIZE'][i] < 1:
+                raise ValueError(f"CvT: WINDOW_SIZE must be >= 1 (stage {i}: {spec['WINDOW_SIZE'][i]})")
         total_depth = sum(spec['DEPTH'])
         dpr = [x.item() for x in torch.linspace(0, spec['DROP_PATH_RATE'], total_depth)]
         in_chans, depth_accum = 3, 0
@@ -327,6 +327,8 @@ S1_SPEC = dict(INIT='trunc_norm', NUM_STAGES=4, REL_POS_EMBED=False, SHIFT=[Fals
                PATCH_SIZE=[7, 3, 3, 3], PATCH_STRIDE=[4, 2, 2, 2], PATCH_PADDING=[2, 1, 1, 1], WINDOW_SIZE=[7] * 4,
                DIM_EMBED=[64, 192, 384, 768], NUM_HEADS=[1, 3, 6, 12], DEPTH=[2, 2, 6, 2], MLP_RATIO=[4.0] * 4,
                QKV_BIAS=[True] * 4, KERNEL_QKV=[3] * 4, PADDING_QKV=[1] * 4)
+# experiments/imagenet/cvt_v4/win_size/s1.yaml MODEL.SPEC: s1 with 14 x 14 windows in stages 0-2
+S1_W14_SPEC = dict(S1_SPEC, WINDOW_SIZE=[14, 14, 14, 7])
 
 
 def cvt(spec: Optional[dict] = None, num_classes: int = 0, use_dense_prediction: bool = False,

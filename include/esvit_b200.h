@@ -226,8 +226,9 @@ int esvit_vit_split(float* x, float* cls, float* region, int B, int N, int D, in
  *   k x k / stride / pad conv in the weight's (c, ky, kx) order, columns >= C*k*k zero; Kp % 8 == 0.
  * conv_col2im: the transpose: drows bf16 [B*Ho*Wo, Kp] -> dx fp32 token-major [B*H*W, C] (written), fixed-order gather.
  * mhsa_win_fwd / _bwd: esvit_mhsa_fwd / _bwd over the w x w windows of the zero-padded map (Hp, Wp = H, W rounded up to
- *   multiples of w; w*w <= 64): qkv / dqkv bf16 [B*Hp*Wp, 3C], out / dout bf16 [B*H*W, C] (padded rows not stored / read
- *   as zero), lse / dvec fp32 [B * windows, nH, w*w].
+ *   multiples of w; any 1 <= w <= min(H, W), ceil(w*w / 64) query and key tiles per window; B * windows <= 65535 and
+ *   B*Hp*Wp <= INT_MAX): qkv / dqkv bf16 [B*Hp*Wp, 3C], out / dout bf16 [B*H*W, C] (padded rows not stored / read as
+ *   zero), lse / dvec fp32 [B * windows, nH, w*w].
  * dwbn_*: depthwise 3x3 conv (pad 1, no bias; w fp32 [C, 9]) of y bf16 [B*H*W, C] zero-padded to Hp x Wp, then
  *   BatchNorm2d; C % 64 == 0.  fwd_stats: z bf16 [B*Hp*Wp, C] (conv output), sums fp64 [2C + 1] = (sum z, sum z^2, count).
  *   fwd_apply: stat fp32 [4C] = (mean, rstd, gamma rstd, beta - mean gamma rstd) from sums (train: run_mean / run_var /
