@@ -253,14 +253,15 @@ __global__ void __launch_bounds__(256) normalize_rows_kernel(const float* __rest
 }
 
 // CTA (b, iq): the teacher view's Tg normalised region features stream through shared memory in chunks of TC rows
-// (one chunk whenever all Tg * P fit, which covers every Swin shape; ViT at Tg = 196 needs several); each warp takes
+// (one chunk whenever all Tg * P fit, which covers Swin-T/S/B; ViT at Tg = 196 and Swin-L's 49 x 1536 need several); each warp takes
 // student tokens of every crop v != iq, computes the cosine similarities (fp32, warp-reduced dot) and keeps the FIRST
 // maximal index (torch.max tie rule, main_esvit.py:736).  Across chunks the running maximum and its index are kept in
 // shared memory per token; the dot order and the strict > are those of a single pass, so the indices do not depend on TC.
 //   sn rows: crop v<2 at (v*B + b)*Tg + i ; crop v>=2 at 2*B*Tg + ((v-2)*B + b)*Tl + i
 //   tn rows: (iq*B + b)*Tg + j
 //   idx out: int64 [2, ncrops, B, Tg] (unused slots untouched); trow out: int32 [Rs, 2] (-1 where v == iq)
-constexpr int RM_MAXV = 8;  // P <= 1024
+// RM_MAXV float4 of the student row per lane: 8 up to P = 1024 (Swin-T/S/B, ViT, CvT, ViL), 12 up to P = 1536 (Swin-L)
+template <int RM_MAXV>
 __global__ void __launch_bounds__(256) region_match_kernel(const float* __restrict__ sn, const float* __restrict__ tn,
                                                            int B, int ncrops, int Tg, int Tl, int P, int TC,
                                                            long long* __restrict__ idx_out, int* __restrict__ trow) {
@@ -759,7 +760,7 @@ ESVIT_API int esvit_normalize_rows(const float* x, float* y, long long R, int P,
 
 ESVIT_API int esvit_region_match(const float* sn, const float* tn, int B, int ncrops, int Tg, int Tl, int P,
                                  long long* idx_out, int* trow, void* stream) {
-  if (P % 4 != 0 || P > 128 * RM_MAXV || B <= 0 || ncrops < 2) return ESVIT_ERR_BAD_ARG;
+  if (P % 4 != 0 || P > 1536 || B <= 0 || ncrops < 2) return ESVIT_ERR_BAD_ARG;
   const size_t budget = 220 * 1024, row = (size_t)P * sizeof(float);
   const size_t state = (size_t)(2 * Tg + (ncrops - 2) * Tl) * (sizeof(float) + sizeof(int));
   int TC = Tg;  // all teacher rows in one chunk when they fit, else as many as fit beside the running arg-max state
@@ -769,8 +770,9 @@ ESVIT_API int esvit_region_match(const float* sn, const float* tn, int B, int nc
     TC = (int)((budget - state) / row);
     smem = (size_t)TC * row + state;
   }
-  cudaError_t e = cudaFuncSetAttribute(region_match_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  auto kernel = P <= 1024 ? region_match_kernel<8> : region_match_kernel<12>;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
-  region_match_kernel<<<dim3(B, 2), 256, smem, (cudaStream_t)stream>>>(sn, tn, B, ncrops, Tg, Tl, P, TC, idx_out, trow);
+  kernel<<<dim3(B, 2), 256, smem, (cudaStream_t)stream>>>(sn, tn, B, ncrops, Tg, Tl, P, TC, idx_out, trow);
   ESVIT_LAUNCH_CHECK();
 }

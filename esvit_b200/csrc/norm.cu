@@ -282,10 +282,15 @@ __global__ void __launch_bounds__(256) merge_ln_bwd_kernel(
   for (int i = 0; i < NV; i++) { ag[i] = make_float4(0, 0, 0, 0); ab[i] = make_float4(0, 0, 0, 0); }
   for (int i = threadIdx.x; i < 2 * C4; i += blockDim.x) sred[i] = 0.f;
   __syncthreads();
+  // Up to NV = 16 the row's xh and gamma * dy stay in registers from the statistics pass to the dx pass.  At NV = 24
+  // (4C = 3072) the dgamma / dbeta accumulators alone take 192 registers, so the statistics pass keeps nothing and
+  // the dx pass loads the row again (it was just read by this warp: an L1 / L2 hit).
+  constexpr bool HOLD = NV <= 16;
+  constexpr int NH = HOLD ? NV : 1;
   for (long long row = warp; row < T; row += nwarps) {
     const int ox = (int)(row % Wo), oy = (int)((row / Wo) % Ho), b = (int)(row / ((long long)Wo * Ho));
     const float mean = mean_i[row], rstd = rstd_i[row];
-    float4 xh[NV], g[NV];
+    float4 xh[NH], g[NH];
     float s1 = 0.f, s2 = 0.f;
 #pragma unroll
     for (int i = 0; i < NV; i++) {
@@ -297,12 +302,15 @@ __global__ void __launch_bounds__(256) merge_ln_bwd_kernel(
         if (sy < H && sx < W) xv = Vec4IO<float>::ld(x + (((long long)b * H + sy) * W + sx) * C + cc);
         float4 d = Vec4IO<bf16>::ld(dy + row * C4 + c);
         float4 gm = Vec4IO<float>::ld(gamma + c);
-        xh[i] = make_float4((xv.x - mean) * rstd, (xv.y - mean) * rstd, (xv.z - mean) * rstd, (xv.w - mean) * rstd);
-        g[i] = make_float4(d.x * gm.x, d.y * gm.y, d.z * gm.z, d.w * gm.w);
-        s1 += sum4(g[i]);
-        s2 += (g[i].x * xh[i].x + g[i].y * xh[i].y) + (g[i].z * xh[i].z + g[i].w * xh[i].w);
-        ag[i].x += d.x * xh[i].x; ag[i].y += d.y * xh[i].y; ag[i].z += d.z * xh[i].z; ag[i].w += d.w * xh[i].w;
-        ab[i].x += d.x; ab[i].y += d.y; ab[i].z += d.z; ab[i].w += d.w;
+        const int h = HOLD ? i : 0;
+        xh[h] = make_float4((xv.x - mean) * rstd, (xv.y - mean) * rstd, (xv.z - mean) * rstd, (xv.w - mean) * rstd);
+        g[h] = make_float4(d.x * gm.x, d.y * gm.y, d.z * gm.z, d.w * gm.w);
+        s1 += sum4(g[h]);
+        s2 += (g[h].x * xh[h].x + g[h].y * xh[h].y) + (g[h].z * xh[h].z + g[h].w * xh[h].w);
+        if constexpr (HOLD) {
+          ag[i].x += d.x * xh[i].x; ag[i].y += d.y * xh[i].y; ag[i].z += d.z * xh[i].z; ag[i].w += d.w * xh[i].w;
+          ab[i].x += d.x; ab[i].y += d.y; ab[i].z += d.z; ab[i].w += d.w;
+        }
       }
     }
     s1 = warp_sum(s1) * inv;
@@ -313,12 +321,23 @@ __global__ void __launch_bounds__(256) merge_ln_bwd_kernel(
       if (c < C4) {
         const int q = c / C, cc = c - q * C;
         const int sy = 2 * oy + (q & 1), sx = 2 * ox + (q >> 1);
+        if constexpr (!HOLD) {
+          float4 xv = make_float4(0, 0, 0, 0);
+          if (sy < H && sx < W) xv = Vec4IO<float>::ld(x + (((long long)b * H + sy) * W + sx) * C + cc);
+          float4 d = Vec4IO<bf16>::ld(dy + row * C4 + c);
+          float4 gm = Vec4IO<float>::ld(gamma + c);
+          xh[0] = make_float4((xv.x - mean) * rstd, (xv.y - mean) * rstd, (xv.z - mean) * rstd, (xv.w - mean) * rstd);
+          g[0] = make_float4(d.x * gm.x, d.y * gm.y, d.z * gm.z, d.w * gm.w);
+          ag[i].x += d.x * xh[0].x; ag[i].y += d.y * xh[0].y; ag[i].z += d.z * xh[0].z; ag[i].w += d.w * xh[0].w;
+          ab[i].x += d.x; ab[i].y += d.y; ab[i].z += d.z; ab[i].w += d.w;
+        }
+        const int h = HOLD ? i : 0;
         if (sy < H && sx < W) {
           float4 o;
-          o.x = rstd * (g[i].x - s1 - xh[i].x * s2);
-          o.y = rstd * (g[i].y - s1 - xh[i].y * s2);
-          o.z = rstd * (g[i].z - s1 - xh[i].z * s2);
-          o.w = rstd * (g[i].w - s1 - xh[i].w * s2);
+          o.x = rstd * (g[h].x - s1 - xh[h].x * s2);
+          o.y = rstd * (g[h].y - s1 - xh[h].y * s2);
+          o.z = rstd * (g[h].z - s1 - xh[h].z * s2);
+          o.w = rstd * (g[h].w - s1 - xh[h].w * s2);
           Vec4IO<float>::st(dx + (((long long)b * H + sy) * W + sx) * C + cc, o);
         }
       }
@@ -376,6 +395,7 @@ int row_grid(long long T, int warps_per_block, int waves) {
   else if ((C_) <= 512) { CALL(4) }            \
   else if ((C_) <= 1024) { CALL(8) }           \
   else if ((C_) <= 2048) { CALL(16) }          \
+  else if ((C_) <= 3072) { CALL(24) }          \
   else return ESVIT_ERR_BAD_ARG;
 
 // (lanes per row, float4 chunks per lane) for a row of C floats

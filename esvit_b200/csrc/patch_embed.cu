@@ -407,17 +407,27 @@ ESVIT_API int esvit_patch_embed_fwd(const float* img, const float* w, const floa
                                     const float* beta, float eps, float* out, float* mean, float* rstd, int B, int H,
                                     int W, int E, void* stream) {
   if (H % 4 || W % 4 || B <= 0) return ESVIT_ERR_BAD_ARG;
-  if (E % 16 == 0 && E <= 128 && E >= 32) {  // register-tiled v2
+  if (E % 16 == 0 && E <= 192 && E >= 32) {  // register-tiled v2
     const long long T = (long long)B * (H / 4) * (W / 4);
     long long need = (T + PE_TM - 1) / PE_TM, cap = (long long)esvit_num_sms() * 4;
     const int grid2 = (int)(need < cap ? need : cap);
     const size_t smem2 = (size_t)(PE_K * E + PE_K * PE_LDA) * sizeof(float);
-#define CALL2(EJ) patch_embed_fwd2_kernel<EJ><<<grid2, 256, smem2, (cudaStream_t)stream>>>(img, w, bias, gamma, beta, eps, out, mean, rstd, B, H, W);
+#define CALL2(EJ)                                                                                                  \
+  {                                                                                                                \
+    if (smem2 > 48 * 1024) { /* E = 192 */                                                                        \
+      cudaError_t e2 = cudaFuncSetAttribute(patch_embed_fwd2_kernel<EJ>,                                           \
+                                            cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2);              \
+      if (e2 != cudaSuccess) return (int)e2;                                                                       \
+    }                                                                                                              \
+    patch_embed_fwd2_kernel<EJ><<<grid2, 256, smem2, (cudaStream_t)stream>>>(img, w, bias, gamma, beta, eps, out,  \
+                                                                             mean, rstd, B, H, W);                 \
+  }
     switch (E / 16) {
       case 2: CALL2(2) break;
       case 4: CALL2(4) break;
       case 6: CALL2(6) break;
       case 8: CALL2(8) break;
+      case 12: CALL2(12) break;
       default: return ESVIT_ERR_BAD_ARG;
     }
 #undef CALL2
@@ -439,7 +449,7 @@ ESVIT_API int esvit_patch_embed_bwd(const float* img, const float* w, const floa
                                     const float* mean, const float* rstd, const float* dout, float* dw, float* dbias,
                                     float* dgamma, float* dbeta, int B, int H, int W, int E, void* stream) {
   if (H % 4 || W % 4 || B <= 0) return ESVIT_ERR_BAD_ARG;
-  if (E % 16 == 0 && E <= 128 && E >= 32) {  // register-tiled v2
+  if (E % 16 == 0 && E <= 192 && E >= 32) {  // register-tiled v2
     const long long T = (long long)B * (H / 4) * (W / 4);
     long long need = (T + PE_TM - 1) / PE_TM, cap = (long long)esvit_num_sms() * 2;
     const int grid2 = (int)(need < cap ? need : cap);
@@ -457,6 +467,7 @@ ESVIT_API int esvit_patch_embed_bwd(const float* img, const float* w, const floa
       case 4: CALL2(4) break;
       case 6: CALL2(6) break;
       case 8: CALL2(8) break;
+      case 12: CALL2(12) break;
       default: return ESVIT_ERR_BAD_ARG;
     }
 #undef CALL2

@@ -28,10 +28,12 @@ from .vision_transformer import DINOHead
 
 SWIN_SPECS = {
     "swin_tiny_w7": dict(embed_dim=96, depths=[2, 2, 6, 2], num_heads=[3, 6, 12, 24], window_size=7, drop_path_rate=0.1),
+    "swin_tiny_w14": dict(embed_dim=96, depths=[2, 2, 6, 2], num_heads=[3, 6, 12, 24], window_size=14, drop_path_rate=0.1),
     "swin_small_w7": dict(embed_dim=96, depths=[2, 2, 18, 2], num_heads=[3, 6, 12, 24], window_size=7, drop_path_rate=0.2),
     "swin_small_w14": dict(embed_dim=96, depths=[2, 2, 18, 2], num_heads=[3, 6, 12, 24], window_size=14, drop_path_rate=0.2),
     "swin_base_w7": dict(embed_dim=128, depths=[2, 2, 18, 2], num_heads=[4, 8, 16, 32], window_size=7, drop_path_rate=0.2),
     "swin_base_w14": dict(embed_dim=128, depths=[2, 2, 18, 2], num_heads=[4, 8, 16, 32], window_size=14, drop_path_rate=0.2),
+    "swin_large_w7": dict(embed_dim=192, depths=[2, 2, 18, 2], num_heads=[6, 12, 24, 48], window_size=7, drop_path_rate=0.2),
 }
 # ViT / DeiT (main_esvit.py:304-327): `vit_arch` names the factory in esvit_b200.vision_transformer
 VIT_SPECS = {
