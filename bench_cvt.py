@@ -1,5 +1,6 @@
-"""CvT-13 pre-training step on one GPU: spec s1 (--arch cvt_13, windows 7) or win_size/s1 (--arch cvt_13_w14, windows
-14, 14, 14, 7), 2 x 224^2 + 8 x 96^2 crops, DDINOLoss (dense), K = 65 536.
+"""CvT pre-training step on one GPU: CvT-13 spec s1 (--arch cvt_13, windows 7) or win_size/s1 (--arch cvt_13_w14, windows
+14, 14, 14, 7), spec s3 (--arch cvt_s3, head dim 32, windows 7) or win_size/s3 (--arch cvt_s3_w14), 2 x 224^2 + 8 x
+96^2 crops, DDINOLoss (dense), K = 65 536.
 
     python bench_cvt.py [--arch cvt_13] [--batch 64] [--steps 10] [--warmup 3] [--no-reference]
 
@@ -13,7 +14,7 @@ Prints one JSON line:
   * `kernels`: CUDA-event times per step of the CvT kernels (conv-embed gather / col2im, depthwise + BN forward /
     backward, window attention forward / backward) with their algorithmic bytes (and FLOPs for attention), achieved
     TB/s, and share of the bound the data sheet gives (the larger of FLOPs / 989 TFLOP/s and bytes / 3.35 TB/s), from
-    an eager step; for cvt_13_w14 also `attention_by_L`, the window attention split by tokens per window L = w^2;
+    an eager step; for every arch but cvt_13 also `attention_by_L`, the window attention split by tokens per window L = w^2;
   * `gpu`: card name, power limit and maximum SM clock, read in the same run.
 Nothing is written to the tree.
 """
@@ -153,7 +154,7 @@ class _ReferenceStep:
     """main_esvit.py:280-301 (CvT student / teacher with DINOHeads) and :541-590 (autocast bf16 forward + loss,
     loss.item(), backward, clip_gradients, cancel_gradients_last_layer, AdamW step, EMA) on the unmodified modules."""
 
-    def __init__(self, spec: dict):
+    def __init__(self, spec: dict, drop_path_rate: float):
         from oracle import reference_import as RI
         import torch.distributed as dist
         ns = RI.load()
@@ -171,10 +172,10 @@ class _ReferenceStep:
         def build(dpr):   # get_cls_model (:685-707) without the yacs config
             return ref_cvt.CvT(num_classes=0, act_layer=ref_cvt.QuickGELU, norm_layer=partial(ref_cvt.LayerNorm, eps=1e-5),
                                init="trunc_norm", use_dense_prediction=True, spec=dict(spec, DROP_PATH_RATE=dpr))
-        self.student, self.teacher = build(0.1), build(0.0)
+        self.student, self.teacher = build(drop_path_rate), build(0.0)
         for m in (self.student, self.teacher):   # main_esvit.py never calls .eval(): BatchNorm in train mode
-            m.head = ns.DINOHead(768, K)
-            m.head_dense = ns.DINOHead(768, K)
+            m.head = ns.DINOHead(spec["DIM_EMBED"][-1], K)
+            m.head_dense = ns.DINOHead(spec["DIM_EMBED"][-1], K)
             m.cuda().train()
         self.teacher.load_state_dict(self.student.state_dict())
         for p in self.teacher.parameters():
@@ -209,12 +210,17 @@ class _ReferenceStep:
 
 def run_reference(arch: str, B: int, steps: int, warmup: int) -> dict:
     from esvit_b200.engine import CVT_SPECS
-    ref = _ReferenceStep(CVT_SPECS[arch]["cvt_spec"])
+    ref = _ReferenceStep(CVT_SPECS[arch]["cvt_spec"], CVT_SPECS[arch]["drop_path_rate"])
     imgs = crops(B)
     for _ in range(warmup):
         ref.step(imgs)
     ms = _timed(lambda: ref.step(imgs), steps)
     return {"ms_per_step": round(ms, 2), "images_per_s": round(B / ms * 1e3, 1), "precision": "bf16 autocast"}
+
+
+# arch -> the model and yaml spec named in the metric
+SPEC_NAMES = {"cvt_13": "CvT-13 (s1)", "cvt_13_w14": "CvT-13 (win_size/s1)", "cvt_s3": "CvT (s3)",
+              "cvt_s3_w14": "CvT (win_size/s3)"}
 
 
 def largest_fitting(fn, batches):
@@ -230,7 +236,7 @@ def largest_fitting(fn, batches):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--arch", choices=("cvt_13", "cvt_13_w14"), default="cvt_13")
+    ap.add_argument("--arch", choices=tuple(SPEC_NAMES), default="cvt_13")
     ap.add_argument("--batch", type=int, default=64)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
@@ -250,8 +256,7 @@ def main():
     else:
         rb, r = largest_fitting(lambda b: run_reference(args.arch, b, args.steps, args.warmup), batches)
         ref = dict(r, batch=rb) if rb is not None else f"not run ({r})"
-    spec = "s1" if args.arch == "cvt_13" else "win_size/s1"
-    line = {"metric": f"multi-crop images/sec, CvT-13 ({spec}) pretrain step (2 global 224^2 + 8 local 96^2 crops, "
+    line = {"metric": f"multi-crop images/sec, {SPEC_NAMES[args.arch]} pretrain step (2 global 224^2 + 8 local 96^2 crops, "
                       "DDINOLoss, K=65536)",
             "value": ours["images_per_s"] if B else None, "unit": "images/s", "batch": B,
             "steps": args.steps, "warmup": args.warmup, "ours": ours, "reference": ref, "gpu": gpu_info()}

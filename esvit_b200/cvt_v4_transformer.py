@@ -1,5 +1,5 @@
-"""CvT backbone (models/cvt_v4_transformer.py, specs experiments/imagenet/cvt_v4/s1.yaml and win_size/s1.yaml) behind
-the reference's signatures and state_dict keys.
+"""CvT backbone (models/cvt_v4_transformer.py, specs experiments/imagenet/cvt_v4/s1.yaml, s3.yaml, win_size/s1.yaml and
+win_size/s3.yaml) behind the reference's signatures and state_dict keys.
 
 CvT / get_cls_model take the reference's MODEL.SPEC keys and hold the reference's parameters AND buffers
 (``stage{i}.0.{proj,norm}.*``, ``stage{i}.1.layers.{j}.0.{norm,fn.qkv.dw,fn.qkv.bn,fn.qkv.pw,fn.proj_out}.*``,
@@ -85,7 +85,7 @@ def _sync_group(bn: nn.Module):
 
 
 class Attention(nn.Module):
-    """:108-220 with head dim 64, no rel-pos bias and no shift."""
+    """:108-220 with head dim 64 (s1) or 32 (s3), no rel-pos bias and no shift."""
 
     def __init__(self, dim_in, dim_out, num_heads, qkv_bias, kernel_size, padding, window_size, shift_size,
                  rel_pos_embed, **kwargs):
@@ -193,10 +193,12 @@ class CvT(MultiCropBackbone):
             raise NotImplementedError("CvT: RES_STEM is not implemented")
         if act_layer is not QuickGELU:
             raise NotImplementedError("CvT: the FeedForward activation is QuickGELU (get_cls_model)")
+        # the window attention kernels run head dim 64 (s1) or 32 (s3); one head dim serves every stage of a model
+        head_dims = [spec['DIM_EMBED'][i] / spec['NUM_HEADS'][i] for i in range(self.num_stages)]
+        if len(set(head_dims)) != 1 or head_dims[0] not in (32, 64):
+            raise NotImplementedError("CvT: one head dim per model, 32 or 64 (per stage DIM_EMBED / NUM_HEADS: %s)"
+                                      % ", ".join(f"{d:g}" for d in head_dims))
         for i in range(self.num_stages):
-            dim, heads = spec['DIM_EMBED'][i], spec['NUM_HEADS'][i]
-            if dim != 64 * heads:
-                raise NotImplementedError(f"CvT: head dim 64 only (stage {i}: dim {dim}, {heads} heads)")
             if spec['KERNEL_QKV'][i] != 3 or spec['PADDING_QKV'][i] != 1:
                 raise NotImplementedError("CvT: KERNEL_QKV 3 with PADDING_QKV 1 only")
             if spec['WINDOW_SIZE'][i] < 1:
@@ -329,6 +331,13 @@ S1_SPEC = dict(INIT='trunc_norm', NUM_STAGES=4, REL_POS_EMBED=False, SHIFT=[Fals
                QKV_BIAS=[True] * 4, KERNEL_QKV=[3] * 4, PADDING_QKV=[1] * 4)
 # experiments/imagenet/cvt_v4/win_size/s1.yaml MODEL.SPEC: s1 with 14 x 14 windows in stages 0-2
 S1_W14_SPEC = dict(S1_SPEC, WINDOW_SIZE=[14, 14, 14, 7])
+# experiments/imagenet/cvt_v4/s3.yaml MODEL.SPEC (head dim 32 in every stage)
+S3_SPEC = dict(INIT='trunc_norm', NUM_STAGES=4, REL_POS_EMBED=False, SHIFT=[False] * 4, DROP_PATH_RATE=0.2,
+               PATCH_SIZE=[7, 3, 3, 3], PATCH_STRIDE=[4, 2, 2, 2], PATCH_PADDING=[2, 1, 1, 1], WINDOW_SIZE=[7] * 4,
+               DIM_EMBED=[64, 128, 256, 512], NUM_HEADS=[2, 4, 8, 16], DEPTH=[2, 2, 10, 4], MLP_RATIO=[4.0] * 4,
+               QKV_BIAS=[True] * 4, KERNEL_QKV=[3] * 4, PADDING_QKV=[1] * 4)
+# experiments/imagenet/cvt_v4/win_size/s3.yaml MODEL.SPEC: s3 with 14 x 14 windows in stages 0-2
+S3_W14_SPEC = dict(S3_SPEC, WINDOW_SIZE=[14, 14, 14, 7])
 
 
 def cvt(spec: Optional[dict] = None, num_classes: int = 0, use_dense_prediction: bool = False,

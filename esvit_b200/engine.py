@@ -43,11 +43,13 @@ VIT_SPECS = {
     "vit_base_p16": dict(vit_arch="vit_base", patch_size=16, drop_path_rate=0.1),
 }
 
-# CvT (main_esvit.py:280-301 with experiments/imagenet/cvt_v4/s1.yaml, and win_size/s1.yaml for cvt_13_w14):
-# `cvt_spec` is the MODEL.SPEC
+# CvT (main_esvit.py:280-301 with experiments/imagenet/cvt_v4/s1.yaml, and win_size/s1.yaml for cvt_13_w14; s3.yaml
+# and win_size/s3.yaml for cvt_s3 / cvt_s3_w14): `cvt_spec` is the MODEL.SPEC
 CVT_SPECS = {
     "cvt_13": dict(cvt_spec=cvts.S1_SPEC, drop_path_rate=0.1),
     "cvt_13_w14": dict(cvt_spec=cvts.S1_W14_SPEC, drop_path_rate=0.1),
+    "cvt_s3": dict(cvt_spec=cvts.S3_SPEC, drop_path_rate=0.2),
+    "cvt_s3_w14": dict(cvt_spec=cvts.S3_W14_SPEC, drop_path_rate=0.2),
 }
 
 # Vision Longformer (main_esvit.py:257-276 with the README's vil_2262 arch): `vil_spec` holds MsViT's arguments

@@ -1286,9 +1286,10 @@ class HeadBnGeluFn(Function):
 
 
 class MhsaWinGroupsFn(Function):
-    """Window attention of CvT (Attention.forward :180-218; no mask, no bias) at head dim 64: qkv bf16 [Tp, 3C] of the
-    padded maps (pw GEMM output incl. bias) -> the cropped output bf16 [T, C]; groups as DwBnFn's.  One launch per group.
-    qkv_bias only receives its gradient: the fixed-order column sums of dqkv."""
+    """Window attention of CvT (Attention.forward :180-218; no mask, no bias) at head dim 64 or 32 (C / num_heads; the
+    kernels dispatch on it): qkv bf16 [Tp, 3C] of the padded maps (pw GEMM output incl. bias) -> the cropped output bf16
+    [T, C]; groups as DwBnFn's.  One launch per group.  qkv_bias only receives its gradient: the fixed-order column sums
+    of dqkv."""
 
     @staticmethod
     def forward(ctx, qkv, qkv_bias, groups, num_heads: int, scale: float):

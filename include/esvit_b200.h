@@ -227,7 +227,8 @@ int esvit_vit_split(float* x, float* cls, float* region, int B, int N, int D, in
  * conv_col2im: the transpose: drows bf16 [B*Ho*Wo, Kp] -> dx fp32 token-major [B*H*W, C] (written), fixed-order gather.
  * mhsa_win_fwd / _bwd: esvit_mhsa_fwd / _bwd over the w x w windows of the zero-padded map (Hp, Wp = H, W rounded up to
  *   multiples of w; any 1 <= w <= min(H, W), ceil(w*w / 64) query and key tiles per window; B * windows <= 65535 and
- *   B*Hp*Wp <= INT_MAX): qkv / dqkv bf16 [B*Hp*Wp, 3C], out / dout bf16 [B*H*W, C] (padded rows not stored / read as
+ *   B*Hp*Wp <= INT_MAX) at head dim 64 or 32: C = nH*64 or C = nH*32 (else ESVIT_ERR_BAD_ARG), channels
+ *   [q|k|v][head][C / nH]: qkv / dqkv bf16 [B*Hp*Wp, 3C], out / dout bf16 [B*H*W, C] (padded rows not stored / read as
  *   zero), lse / dvec fp32 [B * windows, nH, w*w].
  * dwbn_*: depthwise 3x3 conv (pad 1, no bias; w fp32 [C, 9]) of y bf16 [B*H*W, C] zero-padded to Hp x Wp, then
  *   BatchNorm2d; C % 64 == 0.  fwd_stats: z bf16 [B*Hp*Wp, C] (conv output), sums fp64 [2C + 1] = (sum z, sum z^2, count).
