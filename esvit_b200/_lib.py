@@ -58,7 +58,7 @@ SIGNATURES = {
     "esvit_mixup_q": [P, P, I, I, I, F, P, P, P, P],
     "esvit_colsum_workspace_rows": [],
     "esvit_colsum": [P, L, I, P, P, P],
-    "esvit_center_ema": [P, P, F, F, P, I, P],
+    "esvit_center_ema": [P, P, F, D, P, I, P],
     "esvit_normalize_rows": [P, P, L, I, F, P],
     "esvit_region_match": [P, P, I, I, I, I, I, P, P, P],
     "esvit_mhsa_fwd": [P, P, P, I, I, I, I, F, P],

@@ -183,10 +183,11 @@ int esvit_mixup_q(const float* targets, const void* q, int ncrops, int B, int K,
 /* ---- update_center ----------------------------------------------------------- main_esvit.py:650-660, :752-770
  * colsum: out[k] = sum_r t[r,k] (deterministic two-stage); workspace fp32 [esvit_colsum_workspace_rows()*K].
  * center_ema: center_out = center*m + (colsum/rows_total)*(1-m)  (after the caller's SUM all-reduce of colsum);
- * out-of-place like the reference's rebinding, because the loss backward still reads the old center. */
+ * out-of-place like the reference's rebinding, because the loss backward still reads the old center.  momentum is the
+ * double the reference holds: m and 1 - m are each rounded to fp32 from it, as ATen rounds a Python scalar. */
 int esvit_colsum_workspace_rows(void);
 int esvit_colsum(const void* t, long long R, int K, float* workspace, float* out, void* stream);
-int esvit_center_ema(const float* center, const float* colsum, float rows_total, float momentum, float* center_out,
+int esvit_center_ema(const float* center, const float* colsum, float rows_total, double momentum, float* center_out,
                      int K, void* stream);
 
 /* ---- DDINOLoss region match -------------------------------------------------------- main_esvit.py:735-736
