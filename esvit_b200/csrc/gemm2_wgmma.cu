@@ -1083,7 +1083,10 @@ ESVIT_API int esvit_gemm_wgrad_ws_floats(int N, int K) {
 }
 ESVIT_API int esvit_gemm_wgrad(const void* dy, const void* x, float* dw, float* ws, long long T, int N, int K,
                                int accumulate, int tile, void* stream) {
-  if (T <= 0 || N <= 0 || K <= 0 || (N % 8) || (K % 8) || T > 0x7fffffffLL || !ws) return ESVIT_ERR_BAD_ARG;
+  if (T <= 0 || N <= 0 || K <= 0 || (N % 8) || (K % 8) || T > 0x7fffffffLL || !dw || !ws) return ESVIT_ERR_BAD_ARG;
+  // the fold reads and writes dw and reads ws as float4
+  auto aligned = [](const void* q) { return ((uintptr_t)q & 15u) == 0; };
+  if (!aligned(dw) || !aligned(ws)) return ESVIT_ERR_BAD_ARG;
   // GEMM view: M = N (out features), N = K (in features), contraction = T
   int wg, bn;
   hg::pick_tile_wgrad(N, K, tile, &wg, &bn);

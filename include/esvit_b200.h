@@ -109,7 +109,8 @@ int esvit_gemm_mul_colsum(const void* a, const void* w, const void* mult, void* 
  *   b_mn = 0 only).  tile: 0 = automatic, else warpgroups * 1000 + BN.
  * gemm_mul_colsum2: out = (a . opB(b)) * mult, colsum ACCUMULATED (see esvit_gemm_mul_colsum); ws fp32 [160 * N].
  * gemm_wgrad: dw[N,K] (fp32) (+)= dy[T,N]^T . x[T,K], split over T, deterministic fold of fp32 partial tiles held in ws
- *   (esvit_gemm_wgrad_ws_floats(N, K) fp32 elements).  All of M / N / K / T multiples of 8. */
+ *   (esvit_gemm_wgrad_ws_floats(N, K) fp32 elements); dw and ws 16-byte aligned (else ESVIT_ERR_BAD_ARG).  All of
+ *   M / N / K / T multiples of 8. */
 int esvit_gemm_bf16(const void* a, const void* b, const float* bias, void* out, void* pre, long long M, int N, int K,
                     int a_mn, int b_mn, int act, int tile, void* stream);
 int esvit_gemm_mul_colsum2(const void* a, const void* b, const void* mult, void* out, float* colsum, float* ws,
