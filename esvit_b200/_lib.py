@@ -94,6 +94,8 @@ SIGNATURES = {
     "esvit_clip_multi": [P, P, I, F, P, P, P],
     "esvit_grad_sumsq_multi": [P, P, I, P, P],
     "esvit_adamw_ema_multi": [P, P, P, P, P, P, P, P, I, P, P, P, P],
+    "esvit_lars_sums_multi": [P, P, P, I, P, P],
+    "esvit_sgd_ema_multi": [P, P, P, P, P, P, P, I, P, P, P, P],
     "esvit_knn_prep": [P, P, P, P, L, L, I, P],
     "esvit_knn_select": [P, L, P, P, P, P, P, I, I, I, I, I, P, P, P, P, P, P],
     "esvit_knn_vote": [P, P, P, P, L, I, F, I, P, P],
@@ -257,8 +259,12 @@ def call(name: str, *args) -> None:  # noqa: F811  (instrumented wrapper)
         _launch_count += 2 * ((args[2] + 63) // 64)
     elif name == "esvit_grad_sumsq_multi":
         _launch_count += (args[2] + 63) // 64
+    elif name == "esvit_lars_sums_multi":
+        _launch_count += (args[3] + 63) // 64
     elif name == "esvit_adamw_ema_multi":
         _launch_count += (args[8] + 31) // 32 + 1
+    elif name == "esvit_sgd_ema_multi":
+        _launch_count += (args[7] + 31) // 32 + 1
     else:
         _launch_count += _LAUNCHES.get(name, 1)
     if name in _timed_names:

@@ -3,7 +3,8 @@ through the esvit_b200 modules.  ``main_esvit.py`` can keep its own loop (INTEGR
 sequence packaged for bench.py / smoke / tests:
 
     lr/wd -> teacher fwd (no grad) -> student fwd -> DINO/DDINO loss (+ packed center all-reduce) -> backward
-    (DDP gradient all-reduce when wrapped) -> per-tensor clip -> cancel last-layer grads -> AdamW -> teacher EMA
+    (DDP gradient all-reduce when wrapped) -> per-tensor clip -> cancel last-layer grads -> AdamW / SGD / LARS
+    -> teacher EMA
 
 with NO host synchronisation inside the step (the reference syncs ~190 times per step, SURVEY.md §3.5).
 """
@@ -19,7 +20,7 @@ import torch.distributed as dist
 
 from . import ops, utils
 from .losses import DDINOLoss, DINOLoss, mixup_targets
-from .optim import FusedAdamWEMA
+from .optim import FusedAdamWEMA, FusedSGDEMA
 from . import cvt_v4_transformer as cvts
 from . import vision_longformer as vils
 from . import vision_transformer as vits
@@ -144,9 +145,9 @@ class _GradReducer:
 
 class SelfDistillStep:
     """One training step.  optimizer: a torch optimizer (the reference's own sequence: clip kernel, cancel grads,
-    optimizer.step(), EMA kernel) or an esvit_b200.optim.FusedAdamWEMA (clip + AdamW + EMA in one sweep).
-    With use_cuda_graph=True (FusedAdamWEMA only) the whole step - teacher fwd, student fwd/bwd, loss, center update,
-    gradient all-reduce, optimiser sweep - is captured once per (teacher_temp, last-layer-frozen) state and replayed:
+    optimizer.step(), EMA kernel) or an esvit_b200.optim.FusedAdamWEMA / FusedSGDEMA (clip + AdamW / SGD / LARS + EMA
+    in one sweep).  With use_cuda_graph=True (fused optimisers only) the whole step - teacher fwd, student fwd/bwd,
+    loss, center update, gradient all-reduce, optimiser sweep - is captured once per (teacher_temp, last-layer-frozen) state and replayed:
     no Python / launch overhead in the steady state.  lr / wd / momentum live in device memory and are refreshed with
     an 32-byte async copy before each replay."""
 
@@ -156,7 +157,7 @@ class SelfDistillStep:
         self.student, self.teacher, self.loss, self.opt = student, teacher, loss, optimizer
         self.student_call = student_ddp if student_ddp is not None else student
         self.clip_grad, self.freeze_last_layer = clip_grad, freeze_last_layer
-        self.fused = isinstance(optimizer, FusedAdamWEMA)
+        self.fused = isinstance(optimizer, (FusedAdamWEMA, FusedSGDEMA))
         self.use_cuda_graph = use_cuda_graph and self.fused
         self.grad_allreduce = grad_allreduce  # own flat all-reduce of the gradients (used instead of DDP in graph mode)
         self.last_norms = None
@@ -194,7 +195,7 @@ class SelfDistillStep:
             ops.end_step()
         self.reduce_gradients()
         if self.fused:
-            self.opt.step()  # clip + AdamW + EMA, one sweep
+            self.opt.step()  # clip + AdamW / SGD / LARS + EMA, one sweep
         else:
             if self.clip_grad:
                 self.last_norms = utils.clip_gradients(self.student, self.clip_grad)
@@ -323,9 +324,16 @@ def make_step(arch: str = "swin_tiny_w7", out_dim: int = 65536, ncrops: int = 10
               device: str = "cuda", lr: float = 5e-4, weight_decay: float = 0.04, clip_grad: float = 3.0,
               freeze_last_layer: int = 1, drop_path: Optional[float] = None, img_size: int = 224,
               head_kwargs: Optional[dict] = None, spec: Optional[dict] = None, ddp: bool = False,
-              teacher_temp: float = 0.04, seed: int = 0, optimizer: str = "fused", cuda_graph: bool = False):
+              teacher_temp: float = 0.04, seed: int = 0, optimizer: str = "fused", cuda_graph: bool = False,
+              optimizer_type: str = "adamw"):
     """Build student/teacher/loss/optimizer the way train_esvit does (main_esvit.py:235-435) and return
-    (step, student, teacher, loss)."""
+    (step, student, teacher, loss).  optimizer_type is main_esvit.py's ``--optimizer`` (adamw | sgd | lars);
+    optimizer picks the implementation: "fused" (FusedAdamWEMA / FusedSGDEMA) or "torch" (the reference's own
+    torch.optim.AdamW / torch.optim.SGD objects; utils.LARS has no torch counterpart here)."""
+    if optimizer_type not in ("adamw", "sgd", "lars"):
+        raise ValueError(f"optimizer_type must be adamw, sgd or lars, not {optimizer_type!r}")
+    if optimizer != "fused" and optimizer_type == "lars":
+        raise ValueError("optimizer_type='lars' runs on the fused sweep only: use optimizer='fused'")
     if spec is None:
         spec = VIT_SPECS.get(arch) or CVT_SPECS.get(arch) or VIL_SPECS.get(arch) or SWIN_SPECS[arch]
     spec = dict(spec)
@@ -348,8 +356,13 @@ def make_step(arch: str = "swin_tiny_w7", out_dim: int = 65536, ncrops: int = 10
     if optimizer == "fused":
         for p in teacher.parameters():
             p.requires_grad = False
-        opt = FusedAdamWEMA(student, teacher, clip_grad=clip_grad)
-    else:  # the reference's own optimizer object (main_esvit.py:410-415)
+        if optimizer_type == "adamw":
+            opt = FusedAdamWEMA(student, teacher, clip_grad=clip_grad)
+        else:
+            opt = FusedSGDEMA(student, teacher, lars=(optimizer_type == "lars"), clip_grad=clip_grad)
+    elif optimizer_type == "sgd":  # the reference's own optimizer objects (main_esvit.py:410-415)
+        opt = torch.optim.SGD(utils.get_params_groups(student), lr=0, momentum=0.9)
+    else:
         opt = torch.optim.AdamW(utils.get_params_groups(student), fused=True)
     step = SelfDistillStep(student, teacher, loss, opt, clip_grad, freeze_last_layer, student_ddp,
                            use_cuda_graph=cuda_graph, grad_allreduce=(optimizer == "fused" and multi))

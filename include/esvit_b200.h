@@ -340,6 +340,19 @@ int esvit_adamw_ema_multi(void* const* params, const void* const* grads, void* c
                           void* const* teacher, void* const* param_bf16, void* const* teacher_bf16,
                           const long long* numel, int n, const float* hyper, float* state, const double* sumsq,
                           void* stream);
+/* SGD-momentum / LARS counterpart of adamw_ema_multi (main_esvit.py:412-415), same conventions:
+ * lars_sums_multi: sums double[3n] (zeroed inside), planar {sum g^2 | sum p^2 | sum g*p}; params (array or entries) may
+ *   be NULL, then only sum g^2 of that tensor is formed.  SGD uses grad_sumsq_multi instead.
+ * sgd_ema_multi: per-tensor clip, coupled weight decay d = c*g + wd*p, LARS trust ratio, momentum buffer
+ *   buf = momentum*buf + d (torch.optim.SGD dampening 0 / utils.LARS mu), p -= lr*buf, teacher EMA, bf16 shadows.
+ *   hyper fp32[8] = {lr, wd(group 0), momentum, eta, ema_m, 1-ema_m, clip(<=0: off), unused};
+ *   state fp32[2n] = per tensor {steps taken, flags: bit0 weight-decayed, bit1 skip, bit2 LARS trust ratio (p.dim()!=1)};
+ *   sums = grad_sumsq_multi's double[n], or lars_sums_multi's double[3n] when any bit2 is set. */
+int esvit_lars_sums_multi(const void* const* grads, const void* const* params, const long long* numel, int n,
+                          double* sums, void* stream);
+int esvit_sgd_ema_multi(void* const* params, const void* const* grads, void* const* momentum_buf, void* const* teacher,
+                        void* const* param_bf16, void* const* teacher_bf16, const long long* numel, int n,
+                        const float* hyper, float* state, const double* sums, void* stream);
 
 /* ---- exact weighted k-NN classifier over frozen features ---------------------------------------- eval_knn.py:193-232
  * knn_prep: xb bf16 [R_pad, D] = bf16(x fp32 [R, D]) with rows >= R zero; norm fp32 [R] = ||x_r||; max_norm fp32 [1]
