@@ -33,8 +33,7 @@ HBM_PEAK = 3.35e12
 BF16_PEAK = 989e12
 CASES_FILE = os.path.join(ROOT, "bench_gemm_cases.json")
 TILES = [0, 1128, 1256, 2128, 2256]
-GEMM_ENTRIES = ["esvit_gemm_bf16", "esvit_gemm_bias_act", "esvit_gemm_mul_colsum2", "esvit_gemm_mul_colsum",
-                "esvit_gemm_wgrad"]
+GEMM_ENTRIES = ["esvit_gemm_bf16", "esvit_gemm_mul_colsum2", "esvit_gemm_wgrad"]
 CLASSES = {"fwd": "forward Linears (bias / GELU + GELU')", "dgrad": "input gradients (MN-major B)",
            "mul": "fc2 input gradient x GELU' + fc1 bias gradient", "wgrad": "weight gradients (fp32 split-K + fold)"}
 
@@ -50,13 +49,8 @@ def case_of(name, a):
         return {"kind": "dgrad" if int(a[9]) else "fwd", "M": int(a[5]), "N": int(a[6]), "K": int(a[7]), "a_mn": int(a[8]),
                 "b_mn": int(a[9]), "act": int(a[10]), "bias": _set(a[2]),
                 "pre": int(a[10]) != 0 and _set(a[4])}
-    if name == "esvit_gemm_bias_act":
-        return {"kind": "fwd", "M": int(a[5]), "N": int(a[6]), "K": int(a[7]), "a_mn": 0, "b_mn": 0, "act": int(a[8]),
-                "bias": _set(a[2]), "pre": int(a[8]) != 0 and _set(a[4])}
     if name == "esvit_gemm_mul_colsum2":
         return {"kind": "mul", "M": int(a[6]), "N": int(a[7]), "K": int(a[8]), "b_mn": int(a[9])}
-    if name == "esvit_gemm_mul_colsum":
-        return {"kind": "mul", "M": int(a[6]), "N": int(a[7]), "K": int(a[8]), "b_mn": 0}
     if name == "esvit_gemm_wgrad":
         return {"kind": "wgrad", "T": int(a[4]), "N": int(a[5]), "K": int(a[6]), "accumulate": int(a[7])}
     raise KeyError(name)

@@ -30,23 +30,6 @@ class _CastCache:
     def __init__(self):
         self.d: Dict[int, Tensor] = {}
 
-    def __call__(self, p: Optional[Tensor]) -> Optional[Tensor]:
-        if p is None:
-            return None
-        k = id(p)
-        t = self.d.get(k)
-        if t is None:
-            t = self.d[k] = shadow.as_bf16(p)  # optimiser-maintained bf16 shadow when registered, else a cast
-        return t
-
-    def transposed(self, p: Tensor) -> Tensor:
-        """bf16 W^T (contiguous) of a 2-D weight: the K-major operand of the fused input-gradient GEMM (ops.MlpFn)."""
-        k = ("T", id(p))
-        t = self.d.get(k)
-        if t is None:
-            t = self.d[k] = shadow.as_bf16(p, track_grad=False).t().contiguous()
-        return t
-
     def expanded_bias(self, table: Tensor, num_heads: int, ws: int) -> Optional[Tensor]:
         """the rel-pos bias table expanded once per forward call (ops.expand_rel_pos_bias), shared by the crop groups."""
         k = ("B", id(table))
@@ -58,7 +41,7 @@ class _CastCache:
         k = ("ng", id(p))
         t = self.d.get(k)
         if t is None:
-            t = self.d[k] = shadow.as_bf16(p, track_grad=False)
+            t = self.d[k] = shadow.as_bf16(p)  # optimiser-maintained bf16 shadow when registered, else a cast
         return t
 
 

@@ -1133,15 +1133,3 @@ ESVIT_API int esvit_mlp_fwd(const void* x, const void* w1, const float* b1, cons
   }
   return ESVIT_ERR_BAD_ARG;
 }
-
-// ---- first-generation entry points, served by the same kernel family ------------------------------------------------
-// out[M,N] (bf16) = act(a[M,K] @ w[N,K]^T + bias[N]); act 1 = GELU (pre, if not NULL, receives gelu'(pre-activation)).
-ESVIT_API int esvit_gemm_bias_act(const void* a, const void* w, const float* bias, void* out, void* pre, long long M,
-                                  int N, int K, int act, void* stream) {
-  return esvit_gemm_bf16(a, w, bias, out, pre, M, N, K, 0, 0, act, 0, stream);
-}
-// out[M,N] (bf16) = (a[M,K] @ w[N,K]^T) * mult[M,N];  colsum[N] (fp32) += column sums of out; ws fp32 [160 * N].
-ESVIT_API int esvit_gemm_mul_colsum(const void* a, const void* w, const void* mult, void* out, float* colsum, float* ws,
-                                    long long M, int N, int K, void* stream) {
-  return esvit_gemm_mul_colsum2(a, w, mult, out, colsum, ws, M, N, K, 0, 0, stream);
-}

@@ -9,7 +9,7 @@ Every GEMM of a Linear - forward, input gradient, weight gradient - is one esvit
 
 so there are no transposed weight copies, no bf16 -> fp32 gradient cast kernels and no library split-K reductions.  The
 fp32 weight gradient goes straight to the fp32 master parameter; bias gradients are produced by the CONSUMER kernel of the
-layer's output (window attention / residual add + LN / GELU-backward epilogue), see ops.LinearBiasFn.
+layer's output (window attention / residual add + LN / GELU-backward epilogue), see LinearFn.
 
 Reference: Mlp / WindowAttention.qkv / .proj / PatchMerging.reduction (models/swin_transformer.py:21-37, 88-91, 125, 150,
 393-420) and DINOHead (models/vision_transformer.py:385-418)."""
@@ -123,42 +123,46 @@ class MlpFn(Function):
 
 
 class HeadMlpFn(Function):
-    """The 3-layer MLP of DINOHead (models/vision_transformer.py:385-403, 414-415): Linear-GELU-Linear-GELU-Linear, with
-    both GELUs in GEMM epilogues and both GELU backwards (+ their bias gradients) in the next layer's input-gradient
-    GEMM epilogue."""
+    """The MLP of DINOHead without BN (models/vision_transformer.py:385-403, 414-415): n >= 1 Linears with a GELU after
+    every one but the last.  forward(x, wp_1, w16_1, b_1, ..., wp_n, w16_n, b_n) (master weight, its bf16 copy, bias per
+    layer): every GELU in its GEMM's epilogue, and every GELU backward (+ its bias gradient) in the next layer's
+    input-gradient GEMM epilogue.  At n = 1 this computes what LinearColsumFn computes."""
 
     @staticmethod
-    def forward(ctx, x, w1p, w1, b1, w2p, w2, b2, w3p, w3, b3):
+    def forward(ctx, x, *params):
         need = any(ctx.needs_input_grad)  # (grad mode is always off inside Function.forward: needs_input_grad is the signal)
-        if need:
-            h1, p1 = ops.gemm(x, w1, b1, act=1, want_pre=True)
-            h2, p2 = ops.gemm(h1, w2, b2, act=1, want_pre=True)
-        else:
-            h1, p1 = ops.gemm(x, w1, b1, act=1), None
-            h2, p2 = ops.gemm(h1, w2, b2, act=1), None
-        y = ops.gemm(h2, w3, b3)
-        ctx.save_for_backward(x, w1, w2, w3, h1, p1, h2, p2)
-        ctx.shapes = (tuple(w1p.shape), tuple(w2p.shape), tuple(w3p.shape))
+        ws, bs = params[1::3], params[2::3]
+        hs, pres = [x], []
+        for w, b in zip(ws[:-1], bs[:-1]):
+            if need:
+                h, p = ops.gemm(hs[-1], w, b, act=1, want_pre=True)
+            else:
+                h, p = ops.gemm(hs[-1], w, b, act=1), None
+            hs.append(h)
+            pres.append(p)
+        y = ops.gemm(hs[-1], ws[-1], bs[-1])
+        ctx.save_for_backward(*hs, *ws, *pres)
+        ctx.shapes = [tuple(wp.shape) for wp in params[0::3]]
         return y
 
     @staticmethod
     @once_differentiable
     def backward(ctx, g):
-        x, w1, w2, w3, h1, p1, h2, p2 = ctx.saved_tensors
-        s1, s2, s3 = ctx.shapes
+        n = len(ctx.shapes)
+        saved = ctx.saved_tensors
+        hs, ws, pres = saved[:n], saved[n:2 * n], saved[2 * n:]
         g = ops._chk(g, BF16, "g")
-        g3 = g.reshape(-1, g.shape[-1])
-        dev = g.device
-        db3 = ops.colsum(g3)
-        dw3 = ops.gemm_wgrad(g3, h2.reshape(-1, h2.shape[-1])).view(s3)
-        db2 = torch.zeros(s2[0], dtype=F32, device=dev)
-        d2 = ops.gemm_mul_colsum(g3, w3, p2.reshape(-1, p2.shape[-1]), db2, b_mn=True)
-        dw2 = ops.gemm_wgrad(d2, h1.reshape(-1, h1.shape[-1])).view(s2)
-        db1 = torch.zeros(s1[0], dtype=F32, device=dev)
-        d1 = ops.gemm_mul_colsum(d2, w2, p1.reshape(-1, p1.shape[-1]), db1, b_mn=True)
-        dw1 = ops.gemm_wgrad(d1, x.reshape(-1, x.shape[-1])).view(s1)
-        dx = ops.gemm(d1, w1, None, b_mn=True).view(x.shape) if ctx.needs_input_grad[0] else None
-        return dx, dw1, None, db1, dw2, None, db2, dw3, None, db3
+        d = g.reshape(-1, g.shape[-1])
+        grads = [None] * (3 * n)   # (dW, None, db) per layer
+        db = ops.colsum(d)
+        for i in reversed(range(n)):
+            grads[3 * i] = ops.gemm_wgrad(d, hs[i].reshape(-1, hs[i].shape[-1])).view(ctx.shapes[i])
+            grads[3 * i + 2] = db
+            if i:
+                db = torch.zeros(ctx.shapes[i - 1][0], dtype=F32, device=g.device)
+                d = ops.gemm_mul_colsum(d, ws[i], pres[i - 1].reshape(-1, pres[i - 1].shape[-1]), db, b_mn=True)
+        dx = ops.gemm(d, ws[0], None, b_mn=True).view(hs[0].shape) if ctx.needs_input_grad[0] else None
+        return (dx, *grads)
 
 
 class LastLayerFn(Function):

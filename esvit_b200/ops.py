@@ -631,64 +631,7 @@ def expand_rel_pos_bias(bias_table: Tensor, num_heads: int, ws: int) -> Optional
     return bws
 
 
-class GeluFn(Function):
-    @staticmethod
-    def forward(ctx, x):
-        x = _chk(x, BF16, "x")
-        y = torch.empty_like(x)
-        _lib.call("esvit_gelu_fwd", _p(x), _p(y), x.numel(), _stream())
-        ctx.save_for_backward(x)
-        return y
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, g):
-        (x,) = ctx.saved_tensors
-        g = _chk(g, BF16, "g")
-        dx = torch.empty_like(x)
-        _lib.call("esvit_gelu_bwd", _p(x), _p(g), _p(dx), x.numel(), _stream())
-        return dx
-
-
-class BiasGeluFn(Function):
-    """y = gelu(x) for x bf16 [..., N] that already holds the producing GEMM's bias; `bias` (fp32 [N] parameter) only
-    receives its gradient = column sums of dx, computed inside the GELU backward kernel."""
-
-    @staticmethod
-    def forward(ctx, x, bias):
-        x = _chk(x, BF16, "x")
-        y = torch.empty_like(x)
-        _lib.call("esvit_gelu_fwd", _p(x), _p(y), x.numel(), _stream())
-        ctx.save_for_backward(x)
-        ctx.bias_meta = (bias.shape, bias.device, bias.data_ptr())
-        return y
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, g):
-        (x,) = ctx.saved_tensors
-        g = _chk(g, BF16, "g")
-        N = x.shape[-1]
-        dx = torch.empty_like(x)
-        db, first = _acc(("bias", ctx.bias_meta[2]), tuple(ctx.bias_meta[0]), ctx.bias_meta[1])
-        _lib.call("esvit_gelu_bwd_dbias", _p(x), _p(g), _p(dx), _p(db), x.numel() // N, N, _stream())
-        return dx, (db if first else None)
-
-
-GEMM_COLSUM_WS_ROWS = 160  # include/esvit_b200.h: esvit_gemm_mul_colsum scratch rows
-
-
-def gemm_bias_act(a: Tensor, w: Tensor, bias: Optional[Tensor], act: int = 0, want_pre: bool = False):
-    """wgmma/TMA GEMM: act(a @ w^T + bias) -> bf16 [M, N] (and gelu'(a @ w^T + bias) when act != 0 and want_pre)."""
-    a, w = _chk(a, BF16, "a"), _chk(w, BF16, "w")
-    bias = _chk(bias, F32, "bias")
-    K = a.shape[-1]
-    M = a.numel() // K
-    N = w.shape[0]
-    out = torch.empty(*a.shape[:-1], N, dtype=BF16, device=a.device)
-    pre = torch.empty_like(out) if (act and want_pre) else None
-    _lib.call("esvit_gemm_bias_act", _p(a), _p(w), _p(bias), _p(out), _p(pre), M, N, K, act, _stream())
-    return (out, pre) if (act and want_pre) else out
+GEMM_COLSUM_WS_ROWS = 160  # include/esvit_b200.h: esvit_gemm_mul_colsum2 scratch rows
 
 
 def gemm(a: Tensor, b: Tensor, bias: Optional[Tensor] = None, act: int = 0, want_pre: bool = False, a_mn: bool = False,
@@ -768,92 +711,6 @@ def gemm_wgrad(dy: Tensor, x: Tensor, out: Optional[Tensor] = None, accumulate: 
     return out
 
 
-class LinearGeluFn(Function):
-    """gelu(x @ w^T + b) as ONE wgmma/TMA kernel (esvit_gemm_bias_act): the GEMM epilogue adds the bias, applies the
-    exact GELU and also emits gelu'(pre-activation), so the [T, 4C] hidden tensor is written once and never re-read in
-    the forward and the backward's dh = dy * gelu' (+ bias gradient) is a pure streaming kernel; dx / dw are library
-    GEMMs."""
-
-    @staticmethod
-    def forward(ctx, x, w, bias):
-        out, pre = gemm_bias_act(x, w, bias, act=1, want_pre=True)
-        ctx.save_for_backward(x, w, pre)
-        ctx.bias_meta = (bias.shape, bias.device, bias.data_ptr())
-        return out
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, g):
-        x, w, pre = ctx.saved_tensors  # pre = gelu'(x @ w^T + b)
-        g = _chk(g, BF16, "g")
-        N = pre.shape[-1]
-        dh = torch.empty_like(pre)
-        db, first = _acc(("bias", ctx.bias_meta[2]), tuple(ctx.bias_meta[0]), ctx.bias_meta[1])
-        _lib.call("esvit_mul_bwd_dbias", _p(pre), _p(g), _p(dh), _p(db), pre.numel() // N, N, _stream())
-        dh2 = dh.reshape(-1, N)
-        dx = (dh2 @ w).view(x.shape) if ctx.needs_input_grad[0] else None
-        dw = dh2.t() @ x.reshape(-1, x.shape[-1]) if ctx.needs_input_grad[1] else None
-        return dx, dw, (db if first else None)
-
-
-
-
-class MlpFn(Function):
-    """fc2(gelu(fc1(x))) of the Swin MLP (models/swin_transformer.py:31-35) with both GELU passes inside wgmma GEMM
-    epilogues.  forward: h, gelu' = esvit_gemm_bias_act(x, w1, b1) (one kernel), y = h @ w2^T + b2 (library GEMM).
-    backward: d(pre) = (dy @ w2) * gelu' and the fc1 bias gradient come out of ONE kernel (esvit_gemm_mul_colsum, w2t =
-    w2^T bf16 [4C, C]); the hidden-sized dh tensor of the unfused chain (GEMM -> multiply kernel) is never written.
-    fc2's bias gradient is produced by the consumer (residual add + LN backward), as for LinearBiasFn."""
-
-    @staticmethod
-    def forward(ctx, x, w1, b1, w2, b2, w2t):
-        h, pre = gemm_bias_act(x, w1, b1, act=1, want_pre=True)
-        with torch.autocast("cuda", enabled=False):
-            y = torch.nn.functional.linear(h, w2, b2)
-        ctx.save_for_backward(x, w1, pre, h, w2t)
-        ctx.bias_meta = (b1.shape, b1.device, b1.data_ptr())
-        return y
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, g):
-        x, w1, pre, h, w2t = ctx.saved_tensors
-        g = _chk(g, BF16, "g")
-        C, N = g.shape[-1], pre.shape[-1]
-        g2 = g.reshape(-1, C)
-        M = g2.shape[0]
-        dw2 = g2.t() @ h.reshape(-1, N) if ctx.needs_input_grad[3] else None
-        dpre = torch.empty_like(pre)
-        db1, first = _acc(("bias", ctx.bias_meta[2]), tuple(ctx.bias_meta[0]), ctx.bias_meta[1])
-        ws = torch.empty(GEMM_COLSUM_WS_ROWS * N, dtype=F32, device=g.device)
-        _lib.call("esvit_gemm_mul_colsum", _p(g2), _p(w2t), _p(pre), _p(dpre), _p(db1), _p(ws), M, N, C, _stream())
-        d2 = dpre.reshape(-1, N)
-        dx = (d2 @ w1).view(x.shape) if ctx.needs_input_grad[0] else None
-        dw1 = d2.t() @ x.reshape(-1, x.shape[-1]) if ctx.needs_input_grad[1] else None
-        return dx, dw1, (db1 if first else None), dw2, None, None
-
-
-class LinearBiasFn(Function):
-    """y = x @ w^T + b as ONE library GEMM (bias in the cuBLASLt epilogue).  The backward produces dx and dw with two
-    library GEMMs and NO bias gradient: the consumer kernel (window attention / GELU / add+LN backward) column-sums
-    it for free, which removes the reference's per-layer `grad.sum(0)` reduction kernels (10 % of the first profile)."""
-
-    @staticmethod
-    def forward(ctx, x, w, b):
-        ctx.save_for_backward(x, w)
-        with torch.autocast("cuda", enabled=False):
-            return torch.nn.functional.linear(x, w, b)
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, g):
-        x, w = ctx.saved_tensors
-        g2 = g.reshape(-1, g.shape[-1])
-        dx = (g2 @ w).view(x.shape) if ctx.needs_input_grad[0] else None
-        dw = g2.t() @ x.reshape(-1, x.shape[-1]) if ctx.needs_input_grad[1] else None
-        return dx, dw, None
-
-
 class L2NormFn(Function):
     @staticmethod
     def forward(ctx, x, eps: float):
@@ -893,12 +750,11 @@ class WeightNormFn(Function):
     @once_differentiable
     def backward(ctx, gw):
         v, g, norm = ctx.saved_tensors
-        f32 = gw.dtype == F32  # fp32 from esvit_gemm_wgrad, bf16 from a library GEMM
-        gw = _chk(gw, F32 if f32 else BF16, "gw")
+        gw = _chk(gw, BF16, "gw")  # autograd hands the gradient over in w's dtype
         K, Dm = v.shape
         dv = torch.empty_like(v)
         dg = torch.empty_like(g) if ctx.needs_input_grad[1] else None
-        _lib.call("esvit_weight_norm_bwd", _p(v), _p(g), _p(norm), _p(gw), 1 if f32 else 0, _p(dv), _p(dg), K, Dm, _stream())
+        _lib.call("esvit_weight_norm_bwd", _p(v), _p(g), _p(norm), _p(gw), _p(dv), _p(dg), K, Dm, _stream())
         return dv, dg
 
 

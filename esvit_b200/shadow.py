@@ -12,7 +12,6 @@ import weakref
 from typing import Dict, Optional, Tuple
 
 import torch
-from torch.autograd import Function
 
 BF16 = torch.bfloat16
 _registry: Dict[int, Tuple[weakref.ref, torch.Tensor, int]] = {}
@@ -41,23 +40,8 @@ def lookup(param: torch.Tensor) -> Optional[torch.Tensor]:
     return shadow
 
 
-class _ShadowCastFn(Function):
-    """Forward: the shadow (no copy).  Backward: routes the bf16 weight gradient to the fp32 master parameter."""
-
-    @staticmethod
-    def forward(ctx, param, shadow):
-        return shadow.view(shadow.shape)
-
-    @staticmethod
-    def backward(ctx, g):
-        return g.float(), None
-
-
-def as_bf16(param: torch.Tensor, track_grad: bool = True) -> torch.Tensor:
-    """bf16 view of a parameter for a GEMM: the registered shadow when there is one, a fresh cast otherwise."""
+def as_bf16(param: torch.Tensor) -> torch.Tensor:
+    """bf16 copy of a parameter for a GEMM, outside autograd (the GEMM's Function routes the fp32 weight gradient to
+    the master parameter): the registered shadow when there is one, a fresh cast otherwise."""
     s = lookup(param)
-    if s is None:
-        return param.to(BF16) if track_grad else param.detach().to(BF16)
-    if track_grad and param.requires_grad and torch.is_grad_enabled():
-        return _ShadowCastFn.apply(param, s)
-    return s
+    return param.detach().to(BF16) if s is None else s

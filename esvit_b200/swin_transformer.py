@@ -14,19 +14,16 @@ Execution model (what differs from the reference, see DESIGN.md):
     trailing add deferred into the following block / PatchMerging / final norm;
   * pad, cyclic shift, window partition/reverse, the relative-position bias gather and the shift mask never
     exist as tensors - the attention kernel derives them from (H, W, window, shift);
-  * the plain GEMMs (qkv, proj, fc1, fc2, reduction) run on the wgmma GEMM family (esvit_b200.linear; library GEMMs
-    with ESVIT_GEMM2=0).
+  * the plain GEMMs (qkv, proj, fc1, fc2, reduction) run on the wgmma GEMM family (esvit_b200.linear).
 """
 from __future__ import annotations
 
 import math
-import os
 from functools import partial
 from typing import List, Optional, Sequence
 
 import torch
 import torch.nn as nn
-import torch.nn.functional as F
 
 from . import backbone, linear, ops, shadow
 from .backbone import MultiCropBackbone, _CastCache
@@ -35,34 +32,15 @@ Tensor = torch.Tensor
 BF16 = torch.bfloat16
 
 
-# fc1 + bias + GELU as one wgmma/TMA GEMM (esvit_gemm_bias_act) instead of library GEMM + GELU kernel
-USE_TCGEN05_FC1 = os.environ.get("ESVIT_TCGEN05_FC1", "1") != "0"
-# every Linear (forward, input gradient, weight gradient) on the wgmma GEMM family (esvit_b200.linear)
-# instead of library GEMMs; ESVIT_GEMM2=0 restores the library-GEMM path of round 1
-USE_GEMM2 = os.environ.get("ESVIT_GEMM2", "1") != "0"
-
-
 def _trunc_normal_(t: Tensor, std: float = .02) -> Tensor:
     return nn.init.trunc_normal_(t, std=std)
 
 
-def _lin(x: Tensor, w: Tensor, b: Optional[Tensor]) -> Tensor:
-    """bf16 library GEMM; fp32 master weights are cast per call (autograd routes the bf16 grads back to fp32)."""
-    with torch.autocast("cuda", enabled=False):
-        return F.linear(x, w.to(BF16), None if b is None else b.to(BF16))
-
-
 def _lin_c(x: Tensor, lin: nn.Linear, cc: Optional[_CastCache]) -> Tensor:
-    """bf16 library GEMM x @ W^T + b (bias in the GEMM epilogue).  The bias GRADIENT is not computed here: the consumer
-    kernel (window attention / GELU / residual add + LN backward) column-sums it, see ops.LinearBiasFn."""
-    if USE_GEMM2:
-        w16 = shadow.as_bf16(lin.weight, track_grad=False) if cc is None else cc.nograd(lin.weight)
-        return linear.LinearFn.apply(x, lin.weight, w16, lin.bias)
-    w = shadow.as_bf16(lin.weight) if cc is None else cc(lin.weight)
-    if lin.bias is None:
-        with torch.autocast("cuda", enabled=False):
-            return F.linear(x, w)
-    return ops.LinearBiasFn.apply(x, w, (shadow.as_bf16(lin.bias, False) if cc is None else cc.nograd(lin.bias)))
+    """x @ W^T + b on the wgmma GEMM family (bias in the GEMM epilogue).  The bias GRADIENT is not computed here: the
+    consumer kernel (window attention / residual add + LN backward) column-sums it, see linear.LinearFn."""
+    w16 = shadow.as_bf16(lin.weight) if cc is None else cc.nograd(lin.weight)
+    return linear.LinearFn.apply(x, lin.weight, w16, lin.bias)
 
 
 def _one_group(x: Tensor):
@@ -84,22 +62,12 @@ class Mlp(nn.Module):
         self.fc2 = nn.Linear(hidden_features, out_features)
 
     def fused(self, x: Tensor, cc: Optional[_CastCache] = None) -> Tensor:
-        """x bf16 [..., C] -> fc2(gelu(fc1(x))) bf16.  fc1.bias gets its gradient from the GELU backward kernel; the
-        caller must route fc2.bias through the residual-add kernel (ops.add_layer_norm / residual_add delta_bias)."""
-        if USE_GEMM2 and self.fc2.bias is not None:
-            cc = cc if cc is not None else _CastCache()
-            return linear.MlpFn.apply(x, self.fc1.weight, cc.nograd(self.fc1.weight), self.fc1.bias, self.fc2.weight,
-                                      cc.nograd(self.fc2.weight), self.fc2.bias)
-        if USE_TCGEN05_FC1:
-            w1 = shadow.as_bf16(self.fc1.weight) if cc is None else cc(self.fc1.weight)
-            if torch.is_grad_enabled() and self.fc1.weight.requires_grad and self.fc2.bias is not None:
-                cc = cc if cc is not None else _CastCache()
-                return ops.MlpFn.apply(x, w1, self.fc1.bias, cc(self.fc2.weight), cc.nograd(self.fc2.bias),
-                                       cc.transposed(self.fc2.weight))
-            h = ops.LinearGeluFn.apply(x, w1, self.fc1.bias)
-        else:
-            h = ops.BiasGeluFn.apply(_lin_c(x, self.fc1, cc), self.fc1.bias)
-        return _lin_c(h, self.fc2, cc)
+        """x bf16 [..., C] -> fc2(gelu(fc1(x))) bf16.  fc1.bias gets its gradient from the fused GELU backward (see
+        linear.MlpFn); the caller must route fc2.bias through the residual-add kernel (ops.add_layer_norm /
+        residual_add delta_bias)."""
+        cc = cc if cc is not None else _CastCache()
+        return linear.MlpFn.apply(x, self.fc1.weight, cc.nograd(self.fc1.weight), self.fc1.bias, self.fc2.weight,
+                                  cc.nograd(self.fc2.weight), self.fc2.bias)
 
     def forward(self, x: Tensor) -> Tensor:
         """Reference signature (standalone use; fc2.bias receives no gradient on this path - use the block)."""

@@ -13,9 +13,10 @@ DINOHead (:384-418): mlp.{0,2,4} Linear(+exact GELU) -> L2 normalise -> weight-n
 bias=False), with parameters ``mlp.N.{weight,bias}``, ``last_layer.weight_g`` [K,1], ``last_layer.weight_v`` [K,D].
 With use_bn=True each hidden Linear is followed by a real nn.BatchNorm1d (``mlp.{1,4}.*``; so utils.has_batchnorms and
 nn.SyncBatchNorm.convert_sync_batchnorm work unchanged) and the MLP runs as ops.HeadBnGeluFn units.
-The three MLP GEMMs and the last-layer GEMM are bf16 library GEMMs; GELU, the row normalisation and the
-weight-norm reparameterisation (fwd + bwd) are esvit_b200 kernels.  Output logits are bf16 [rows, out_dim]
-(what the reference produces under autocast); the losses consume them without an fp32 copy.
+Without BN the MLP of any depth is one linear.HeadMlpFn (GELUs in the GEMM epilogues) and the last layer one
+linear.LastLayerFn; the row normalisation and the weight-norm reparameterisation (fwd + bwd) are esvit_b200 kernels.
+Output logits are bf16 [rows, out_dim] (what the reference produces under autocast); the losses consume them without
+an fp32 copy.
 """
 from __future__ import annotations
 
@@ -31,7 +32,7 @@ from torch.nn.modules.batchnorm import _BatchNorm
 from . import backbone, linear, ops, shadow
 from .backbone import MultiCropBackbone, _CastCache
 from .cvt_v4_transformer import _sync_group
-from .swin_transformer import USE_GEMM2, Mlp, _lin_c
+from .swin_transformer import Mlp, _lin_c
 
 Tensor = torch.Tensor
 
@@ -52,10 +53,7 @@ class _WeightNormLinear(nn.Module):
         return ops.WeightNormFn.apply(self.weight_v, self.weight_g)
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if USE_GEMM2:
-            return linear.LastLayerFn.apply(x, self.effective_weight())
-        with torch.autocast("cuda", enabled=False):
-            return F.linear(x, self.effective_weight())
+        return linear.LastLayerFn.apply(x, self.effective_weight())
 
 
 class DINOHead(nn.Module):
@@ -89,26 +87,14 @@ class DINOHead(nn.Module):
         x = x.to(BF16)
         mods = [self.mlp] if isinstance(self.mlp, nn.Linear) else list(self.mlp)
         if any(isinstance(m, _BatchNorm) for m in mods):
-            return self.last_layer(ops.L2NormFn.apply(self._mlp_bn(x, mods), 1e-12))
-        lins = [m for m in mods if isinstance(m, nn.Linear)]
-        if USE_GEMM2 and len(lins) == 3 and len(mods) == 5:
+            x = self._mlp_bn(x, mods)
+        else:
             args = []
-            for m in lins:
-                args += [m.weight, shadow.as_bf16(m.weight, track_grad=False), m.bias]
+            for m in mods:
+                if isinstance(m, nn.Linear):
+                    args += [m.weight, shadow.as_bf16(m.weight), m.bias]
             x = linear.HeadMlpFn.apply(x, *args)
-            return self.last_layer(ops.L2NormFn.apply(x, 1e-12))
-        with torch.autocast("cuda", enabled=False):
-            for i, m in enumerate(mods):
-                if not isinstance(m, nn.Linear):
-                    continue
-                if i + 1 < len(mods) and isinstance(mods[i + 1], nn.GELU):
-                    # GEMM with bias epilogue; exact GELU kernel whose backward also yields the bias gradient
-                    x = ops.BiasGeluFn.apply(
-                        ops.LinearBiasFn.apply(x, shadow.as_bf16(m.weight), shadow.as_bf16(m.bias, False)), m.bias)
-                else:
-                    x = F.linear(x, shadow.as_bf16(m.weight), shadow.as_bf16(m.bias))
-        x = ops.L2NormFn.apply(x, 1e-12)
-        return self.last_layer(x)
+        return self.last_layer(ops.L2NormFn.apply(x, 1e-12))
 
     @staticmethod
     def _mlp_bn(x: Tensor, mods) -> Tensor:
@@ -117,7 +103,7 @@ class DINOHead(nn.Module):
         i = 0
         while i < len(mods):
             lin = mods[i]
-            w16 = shadow.as_bf16(lin.weight, track_grad=False)
+            w16 = shadow.as_bf16(lin.weight)
             if i + 1 < len(mods) and isinstance(mods[i + 1], _BatchNorm):
                 bn = mods[i + 1]
                 train = bn.training or not bn.track_running_stats
@@ -204,7 +190,7 @@ class PatchEmbed(nn.Module):
         """fp32 crops [B_g, 3, S_g, S_g] -> patch projections bf16 [sum_g B_g N_g, D] (bias included), back to back.
         proj.bias gets its gradient from the consumer (ops.VitTokensGroupsFn)."""
         w = self.proj.weight
-        w16 = (shadow.as_bf16(w, track_grad=False) if cc is None else cc.nograd(w)).view(w.shape[0], -1)
+        w16 = (shadow.as_bf16(w) if cc is None else cc.nograd(w)).view(w.shape[0], -1)
         return linear.LinearFn.apply(ops.vit_patches(imgs, self.patch_size), w, w16, self.proj.bias)
 
     def forward(self, x: Tensor) -> Tensor:

@@ -84,21 +84,6 @@ int esvit_window_attn_bwd(const void* qkv, const void* qkv_bias, const float* bi
 int esvit_window_attn_probs(const void* qkv, const void* qkv_bias, const float* bias_table, float* bias_ws, int bias_ready,
                             float* probs, int B, int H, int W, int C, int nH, int ws, int shift, float scale, void* stream);
 
-/* ---- wgmma / TMA GEMM with fused epilogue --------------------------- nn.Linear + Mlp.act, models/swin_transformer.py:31-33
- * out[M,N] (bf16) = act(a[M,K] @ w[N,K]^T + bias[N]); act 0 = identity, 1 = exact GELU (then `pre`, if not NULL, gets
- * gelu'(pre-activation): the backward is dh = dy * pre, see esvit_mul_bwd_dbias).  a, w bf16 row-major (K contiguous), K % 8 == 0, N % 8 == 0, bias fp32 or NULL.
- * TMA-staged 128B-swizzled tiles, wgmma with the fp32 accumulator in registers, persistent over output tiles. */
-int esvit_gemm_bias_act(const void* a, const void* w, const float* bias, void* out, void* pre, long long M, int N, int K,
-                        int act, void* stream);
-/* out[M,N] (bf16) = (a[M,K] @ w[N,K]^T) * mult[M,N]; colsum[N] (fp32) += column sums of out (caller zero-fills).
- * Same kernel, third epilogue: the fc2 input-gradient GEMM (a = dy, w = W2^T) fused with the GELU backward of fc1
- * (mult = gelu'(pre-activation) from esvit_gemm_bias_act act = 1) and the fc1 bias gradient - what autograd runs as
- * mm + GeluBackward + sum(0) for Mlp.forward, models/swin_transformer.py:31-35.  The epilogue reads the multiplier
- * next to the accumulator fragment it scales.
- * ws fp32 [160*N]: caller-owned scratch (per-CTA partial column sums, folded into colsum inside the call). */
-int esvit_gemm_mul_colsum(const void* a, const void* w, const void* mult, void* out, float* colsum, float* ws,
-                          long long M, int N, int K, void* stream);
-
 /* ---- wgmma GEMM family (csrc/gemm2_wgmma.cu): every nn.Linear of the step, forward, input
  * gradient and weight gradient -------- models/swin_transformer.py:21-37,88-91,125,150,393-420; vision_transformer.py:385-418
  * 64 x BN or 128 x BN tiles (1 or 2 consumer warpgroups, BN 128 / 256); operands K-major or MN-major (the same
@@ -107,7 +92,9 @@ int esvit_gemm_mul_colsum(const void* a, const void* w, const void* mult, void* 
  *   (Linear weight, forward) | b_mn = 1 [K,N] (Linear weight [out = K, in = N], input gradient).  act 0 identity, 1 exact
  *   GELU (pre != NULL also receives gelu'(pre-activation)); act 2: QuickGELU x sigmoid(1.702 x) (pre likewise; a_mn =
  *   b_mn = 0 only).  tile: 0 = automatic, else warpgroups * 1000 + BN.
- * gemm_mul_colsum2: out = (a . opB(b)) * mult, colsum ACCUMULATED (see esvit_gemm_mul_colsum); ws fp32 [160 * N].
+ * gemm_mul_colsum2: out = (a . opB(b)) * mult; colsum[N] (fp32) += column sums of out (caller zero-fills).  The fc2
+ *   input gradient fused with the GELU backward of fc1 (mult = gelu'(pre-activation) from gemm_bf16 act 1) and the fc1
+ *   bias gradient.  ws fp32 [160 * N]: caller-owned scratch (per-CTA partial column sums, folded into colsum).
  * gemm_wgrad: dw[N,K] (fp32) (+)= dy[T,N]^T . x[T,K], split over T, deterministic fold of fp32 partial tiles held in ws
  *   (esvit_gemm_wgrad_ws_floats(N, K) fp32 elements); dw and ws 16-byte aligned (else ESVIT_ERR_BAD_ARG).  All of
  *   M / N / K / T multiples of 8. */
@@ -125,23 +112,14 @@ int esvit_gemm_wgrad(const void* dy, const void* x, float* dw, float* ws, long l
 int esvit_mlp_fwd(const void* x, const void* w1, const float* b1, const void* w2, const float* b2, void* y, void* h,
                   void* gelu_grad, long long M, int C, void* stream);
 
-/* ---- GELU (exact erf), bf16 ------------------------------------------------ models/swin_transformer.py:21-37 */
-int esvit_gelu_fwd(const void* x, void* y, long long n, void* stream);
-int esvit_gelu_bwd(const void* x, const void* dy, void* dx, long long n, void* stream);
-/* gelu backward that also ACCUMULATES dbias fp32 [N] = column sums of dx for x bf16 [R,N]: the gradient of the fc1
- * bias (added by the GEMM epilogue) without a separate reduction kernel. */
-int esvit_gelu_bwd_dbias(const void* x, const void* dy, void* dx, float* dbias, long long R, int N, void* stream);
-/* dx = dy * gp (gp = stored local derivative, bf16 [R,N]); ACCUMULATES dbias fp32 [N] = column sums of dx. */
-int esvit_mul_bwd_dbias(const void* gp, const void* dy, void* dx, float* dbias, long long R, int N, void* stream);
-
 /* ---- DINOHead pieces ------------------------------------------------------ models/vision_transformer.py:403-417
  * l2norm: y = x / max(||x||, eps) rows (bf16); weight_norm: w(bf16) = v * g / ||v||_row (fp32 v [K,D], g [K]). */
 int esvit_l2norm_fwd(const void* x, void* y, float* inv, float eps, long long R, int D, void* stream);
 int esvit_l2norm_bwd(const void* x, const void* dy, const float* inv, void* dx, long long R, int D, void* stream);
 int esvit_weight_norm_fwd(const float* v, const float* g, void* w, float* norm, long long K, int D, void* stream);
-/* dw: bf16 [K,D], or fp32 when dw_is_f32 (the fp32 weight gradient of esvit_gemm_wgrad) */
-int esvit_weight_norm_bwd(const float* v, const float* g, const float* norm, const void* dw, int dw_is_f32, float* dv,
-                          float* dg, long long K, int D, void* stream);
+/* dw: bf16 [K,D], the gradient of w; dv fp32 [K,D]; dg fp32 [K] or NULL */
+int esvit_weight_norm_bwd(const float* v, const float* g, const float* norm, const void* dw, float* dv, float* dg,
+                          long long K, int D, void* stream);
 
 /* ---- DINOLoss / DDINOLoss ---------------------------------------------------- main_esvit.py:620-648, :683-750
  * row_lse: lse[r] = log sum_k exp((x[r,k] - center[k]) * inv_temp)   (center NULL for student rows).

@@ -178,11 +178,16 @@ def forward_features(x: Tensor, sd, spec: SwinSpec, prefix: str = "",
 
 
 def dino_head(x: Tensor, sd, p: str) -> Tensor:
-    """DINOHead.forward, nlayers=3, no BN (models/vision_transformer.py:384-418);
-    weight_norm: w = g * v / ||v||_row (dim=0 default of nn.utils.weight_norm)."""
-    x = F.gelu(linear(x, sd, p + ".mlp.0"))
-    x = F.gelu(linear(x, sd, p + ".mlp.2"))
-    x = linear(x, sd, p + ".mlp.4")
+    """DINOHead.forward, no BN, any nlayers (models/vision_transformer.py:384-418): mlp is one Linear (nlayers 1) or
+    Linear, GELU, ..., Linear; weight_norm: w = g * v / ||v||_row (dim=0 default of nn.utils.weight_norm)."""
+    if p + ".mlp.weight" in sd:
+        x = linear(x, sd, p + ".mlp")
+    else:
+        i = 0
+        while p + f".mlp.{i + 2}.weight" in sd:
+            x = F.gelu(linear(x, sd, f"{p}.mlp.{i}"))
+            i += 2
+        x = linear(x, sd, f"{p}.mlp.{i}")
     x = F.normalize(x, dim=-1, p=2)
     v, g = sd[p + ".last_layer.weight_v"], sd[p + ".last_layer.weight_g"]
     w = v * (g / v.norm(2, dim=1, keepdim=True))

@@ -1,6 +1,6 @@
 """DINOHead(use_bn=True) on the GPU: the BatchNorm1d + GELU kernels (esvit_headbn_*) against fp64 torch, the training
-step against tests/golden/esvit_bnhead.pt (written by the unmodified reference), eval mode, CUDA-graph replay, and the
-unchanged use_bn=False head."""
+step against tests/golden/esvit_bnhead.pt (written by the unmodified reference), eval mode, CUDA-graph replay, the
+unchanged use_bn=False head, and use_bn=False heads of the other depths against fp64."""
 import copy
 
 import pytest
@@ -325,7 +325,38 @@ def test_plain_head_is_unchanged():
         out = h(x)
         args = []
         for m in (h.mlp[0], h.mlp[2], h.mlp[4]):
-            args += [m.weight, shadow.as_bf16(m.weight, track_grad=False), m.bias]
+            args += [m.weight, shadow.as_bf16(m.weight), m.bias]
         y = linear.HeadMlpFn.apply(x.to(BF16), *args)
         want = h.last_layer(ops.L2NormFn.apply(y, 1e-12))
     assert torch.equal(out, want)
+
+
+@pytest.mark.parametrize("nlayers", [1, 2, 4])
+def test_plain_head_any_depth_matches_fp64(nlayers):
+    """DINOHead(use_bn=False, nlayers): one HeadMlpFn of nlayers Linears, the row L2 normalisation and the weight-normed
+    last layer.  The output and the gradients of x, every mlp.* parameter and last_layer.weight_v against fp64 of the
+    reference formula (oracle.swin.dino_head) on the same parameters."""
+    from esvit_b200.vision_transformer import DINOHead
+    from oracle.swin import dino_head
+    torch.manual_seed(nlayers)
+    h = DINOHead(384, 4096, nlayers=nlayers).cuda()
+    gen = _gen(20 + nlayers)
+    with torch.no_grad():
+        for m in h.modules():
+            if isinstance(m, nn.Linear):
+                m.bias.copy_(0.1 * torch.randn(m.bias.shape, generator=gen, device="cuda"))
+    x = torch.randn(640, 384, generator=gen, device="cuda").to(BF16).requires_grad_(True)
+    go = torch.randn(640, 4096, generator=gen, device="cuda").to(BF16)
+    out = h(x)
+    out.backward(go)
+
+    sd = {"h." + k: v.detach().double().requires_grad_(True) for k, v in h.state_dict().items()}
+    x64 = x.detach().double().requires_grad_(True)
+    y = dino_head(x64, sd, "h")
+    y.backward(go.double())
+    assert_close(out, y, TOL_BF16_ACT, "output")
+    assert_close(x.grad, x64.grad, TOL_BF16_GRAD, "dx")
+    names = [k for k, _ in h.named_parameters() if k.startswith("mlp.") or k == "last_layer.weight_v"]
+    assert len(names) == 2 * nlayers + 1
+    for k in names:
+        assert_close(h.get_parameter(k).grad, sd["h." + k].grad, TOL_BF16_GRAD, k)

@@ -161,9 +161,6 @@ def test_n_last_tap_plumbing_at_s3_depths(monkeypatch):
     monkeypatch.setattr(_lib, "call", lambda name, *a: None)
     monkeypatch.setattr(ops, "_stream", lambda: 0)
     monkeypatch.setattr(ops, "_chk", lambda t, dtype, name: None if t is None else t.contiguous())
-    monkeypatch.setattr(ops, "gemm_bias_act", lambda a, w, bias, act=0, want_pre=False: (
-        lambda o: (o, torch.zeros_like(o)) if (act and want_pre) else o)(
-        torch.zeros(*a.shape[:-1], w.shape[0], dtype=torch.bfloat16)))
     torch.manual_seed(0)
     for arch in ("cvt_s3", "cvt_s3_w14"):
         net = engine.build_network(dict(engine.CVT_SPECS[arch]), 256, True, False, True, 224, None).eval()

@@ -1,6 +1,7 @@
 """wgmma / TMA GEMM family (csrc/gemm2_wgmma.cu) against fp32 torch on the same bf16 inputs:
 forward (K-major operands), input gradient (MN-major B = the Linear weight as it lies), weight gradient (MN-major A and
-B, split-K fp32 partials), every epilogue, every tile shape (1 / 2 consumer warpgroups x BN 128 / 256), ragged M / N / K."""
+B, split-K fp32 partials), every epilogue, the automatic tile choice and every tile shape (1 / 2 consumer warpgroups x
+BN 128 / 256), ragged M / N / K."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -9,10 +10,11 @@ from helpers import assert_close
 
 pytestmark = pytest.mark.gpu
 BF16 = torch.bfloat16
-TILES = [1128, 1256, 2128, 2256]  # consumer warpgroups * 1000 + BN
+TILES = [0, 1128, 1256, 2128, 2256]  # 0: the automatic choice; else consumer warpgroups * 1000 + BN
 
 FWD_SHAPES = [(4096, 96, 384), (1000, 192, 768), (300, 384, 1536), (256, 768, 3072), (512, 3072, 768), (777, 64, 96),
-              (128, 128, 288), (33, 96, 288), (20000, 96, 96), (640, 256, 4096), (1111, 2048, 256), (260, 96, 16)]
+              (128, 128, 288), (33, 96, 288), (20000, 96, 96), (640, 256, 4096), (1111, 2048, 256), (260, 96, 16),
+              (340, 768, 256), (340, 2048, 2048)]   # DINO head: a depth-1 head's Linear, a hidden Linear
 
 
 def _mk(M, K, N, seed):
@@ -80,8 +82,8 @@ def test_wgrad_split_k(T, N, K, tile):
 
 @pytest.mark.parametrize("tile", TILES)
 @pytest.mark.parametrize("b_mn", [False, True])
-@pytest.mark.parametrize("M,K,N", [(4096, 96, 384), (1000, 192, 768), (300, 384, 1536), (777, 64, 96), (33, 96, 288),
-                                   (20000, 96, 384), (40000, 128, 512)])
+@pytest.mark.parametrize("M,K,N", [(4096, 96, 384), (1000, 192, 768), (300, 384, 1536), (256, 768, 3072), (777, 64, 96),
+                                   (33, 96, 288), (20000, 96, 384), (40000, 128, 512)])
 def test_mul_colsum(M, K, N, b_mn, tile):
     """out = (a @ w^T) * mult, colsum += column sums (fc2 dgrad fused with the GELU backward), bit-reproducible."""
     from esvit_b200 import ops
@@ -100,11 +102,3 @@ def test_mul_colsum(M, K, N, b_mn, tile):
     out2 = ops.gemm_mul_colsum(a, bop, mult, colsum2, b_mn=b_mn, tile=tile)
     assert torch.equal(out2, out) and torch.equal(colsum2, colsum), "column sums must be bit-reproducible"
 
-
-def test_old_entry_points_still_match():
-    """esvit_gemm_bias_act / esvit_gemm_mul_colsum keep their contracts (now served by the second-generation kernel)."""
-    from esvit_b200 import ops
-    a, w, b = _mk(1000, 192, 768, 3)
-    out, gp = ops.gemm_bias_act(a, w, b, act=1, want_pre=True)
-    ref_pre = a.float() @ w.float().t() + b
-    assert_close(out, F.gelu(ref_pre), 5e-3, "gelu")

@@ -155,25 +155,6 @@ def test_add_layer_norm_with_fused_branch_bias(C):
     assert_close(b3.grad, (keep.view(B, 1, 1) * gx).sum((0, 1)), 1e-4, "add dbias")
 
 
-@pytest.mark.parametrize("R,N", [(77, 384), (1000, 2048), (5, 128)])
-def test_bias_gelu(R, N):
-    from esvit_b200 import ops
-    torch.manual_seed(R + N)
-    x = (torch.randn(R, N) * 2).to(BF16)
-    bias = torch.randn(N) * 0.5
-    g = torch.randn(R, N).to(BF16)
-    xr, br_ = x.float().requires_grad_(True), bias.clone().requires_grad_(True)
-    yr = F.gelu(xr + (br_ - br_.detach()))  # x already contains the bias; the op only produces the bias gradient
-    yr.backward(g.float())
-    d = _dev()
-    xc, bc_ = x.to(d).requires_grad_(True), bias.to(d).requires_grad_(True)
-    y = ops.BiasGeluFn.apply(xc, bc_)
-    y.backward(g.to(d))
-    assert_close(y, yr, 4e-3, "bias gelu")
-    assert_close(xc.grad, xr.grad, 5e-3, "dx")
-    assert_close(bc_.grad, br_.grad, 2e-3, "dbias")
-
-
 def test_token_mean_groups():
     """two resolution groups back to back: 5 maps of 7 x 7, then 3 maps of 3 x 3"""
     from esvit_b200 import ops
@@ -196,15 +177,6 @@ def test_gelu_l2norm_weightnorm():
     x = (torch.randn(64, 256) * 2).to(BF16)
     xr = x.float().requires_grad_(True)
     g = torch.randn(64, 256).to(BF16)
-    yr = F.gelu(xr)
-    yr.backward(g.float())
-    xc = x.to(d).requires_grad_(True)
-    y = ops.GeluFn.apply(xc)
-    y.backward(g.to(d))
-    assert_close(y, yr, 4e-3, "gelu")
-    assert_close(xc.grad, xr.grad, 5e-3, "gelu grad")
-
-    xr = x.float().requires_grad_(True)
     yr = F.normalize(xr, dim=-1, p=2)
     yr.backward(g.float())
     xc = x.to(d).requires_grad_(True)
