@@ -395,6 +395,9 @@ __global__ void __launch_bounds__(256) patch_embed_bwd2_kernel(
 
 }  // namespace
 
+// v2 is instantiated for E / 16 in {2, 4, 6, 8, 12}; every other width up to 128 runs on the first version
+static bool pe_v2(int E) { return E == 32 || E == 64 || E == 96 || E == 128 || E == 192; }
+
 #define PE_DISPATCH(E_, CALL)        \
   if ((E_) <= 32) { CALL(1) }        \
   else if ((E_) <= 64) { CALL(2) }   \
@@ -406,8 +409,8 @@ __global__ void __launch_bounds__(256) patch_embed_bwd2_kernel(
 ESVIT_API int esvit_patch_embed_fwd(const float* img, const float* w, const float* bias, const float* gamma,
                                     const float* beta, float eps, float* out, float* mean, float* rstd, int B, int H,
                                     int W, int E, void* stream) {
-  if (H % 4 || W % 4 || B <= 0) return ESVIT_ERR_BAD_ARG;
-  if (E % 16 == 0 && E <= 192 && E >= 32) {  // register-tiled v2
+  if (H % 4 || W % 4 || B <= 0 || E <= 0) return ESVIT_ERR_BAD_ARG;
+  if (pe_v2(E)) {  // register-tiled v2
     const long long T = (long long)B * (H / 4) * (W / 4);
     long long need = (T + PE_TM - 1) / PE_TM, cap = (long long)esvit_num_sms() * 4;
     const int grid2 = (int)(need < cap ? need : cap);
@@ -448,8 +451,8 @@ ESVIT_API int esvit_patch_embed_fwd(const float* img, const float* w, const floa
 ESVIT_API int esvit_patch_embed_bwd(const float* img, const float* w, const float* bias, const float* gamma,
                                     const float* mean, const float* rstd, const float* dout, float* dw, float* dbias,
                                     float* dgamma, float* dbeta, int B, int H, int W, int E, void* stream) {
-  if (H % 4 || W % 4 || B <= 0) return ESVIT_ERR_BAD_ARG;
-  if (E % 16 == 0 && E <= 192 && E >= 32) {  // register-tiled v2
+  if (H % 4 || W % 4 || B <= 0 || E <= 0) return ESVIT_ERR_BAD_ARG;
+  if (pe_v2(E)) {  // register-tiled v2
     const long long T = (long long)B * (H / 4) * (W / 4);
     long long need = (T + PE_TM - 1) / PE_TM, cap = (long long)esvit_num_sms() * 2;
     const int grid2 = (int)(need < cap ? need : cap);

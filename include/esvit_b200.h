@@ -27,18 +27,23 @@ extern "C" {
  * xout = x + keep[row / tokens_per_sample] * delta (delta/keep/xout may be NULL; delta = proj / fc2 GEMM output
  * including its bias); y = LN(xout) (y may be NULL).  x may be NULL (= 0) when delta is given: xout = fp32(delta), the
  * first LN after PatchMerging's reduction GEMM (:411-415) without a separate bf16 -> fp32 pass.
- * x fp32 [T,C]; delta bf16 [T,C]; keep fp32 [B]; y bf16 or fp32 [T,C]; mean/rstd fp32 [T] (saved for backward). */
+ * x fp32 [T,C]; delta bf16 [T,C]; y bf16 or fp32 [T,C]; mean/rstd fp32 [T] (saved for backward).  keep fp32 has one
+ * entry per tokens_per_sample rows: per sample ([T / tps], tps = tokens of one sample) or per row ([T], tps = 1, the
+ * layout the training step passes).  xout is written only when delta is given.  C % 4 == 0, C <= 2048, T >= 1. */
 int esvit_add_ln_fwd(const float* x, const void* delta, const float* keep, int tokens_per_sample,
                      const float* gamma, const float* beta, float eps, float* xout, void* y, int y_is_bf16,
                      float* mean, float* rstd, long long T, int C, void* stream);
 /* dx = dxo + LNbwd(dy); ddelta = keep * dx (bf16); dgamma/dbeta/ddelta_bias ACCUMULATED (ddelta_bias = column sums of
- * ddelta = gradient of the proj / fc2 bias).  dy / dxo / dx / ddelta / ddelta_bias may be NULL. */
+ * ddelta = gradient of the proj / fc2 bias).  dy / dxo / dx / ddelta / ddelta_bias may be NULL; dy = NULL (a residual
+ * add without norm: dx = dxo) leaves dgamma / dbeta untouched and does not read xs / mean / rstd / gamma. */
 int esvit_add_ln_bwd(const void* dy, int dy_is_bf16, const float* dxo, const float* xs, const float* mean,
                      const float* rstd, const float* gamma, const float* keep, int tokens_per_sample, float* dx,
                      void* ddelta, float* dgamma, float* dbeta, float* ddelta_bias, long long T, int C, void* stream);
 
 /* ---- PatchMerging gather + LayerNorm(4C) ---------------------------------- models/swin_transformer.py:393-417
- * x fp32 [B,H,W,C] -> y bf16 [B,ceil(H/2)*ceil(W/2),4C] (the 4C->2C reduction GEMM follows as a library GEMM). */
+ * x fp32 [B,H,W,C] -> y bf16 [B,ceil(H/2)*ceil(W/2),4C]; odd H / W are zero-padded and the pad counts in the 4C
+ * statistics (the 4C->2C reduction that follows runs on esvit_gemm_bf16).  C % 4 == 0, 4C <= 3072.
+ * bwd: dx written at every real position; dgamma / dbeta [4C] ACCUMULATED. */
 int esvit_patch_merge_ln_fwd(const float* x, const float* gamma, const float* beta, float eps, void* y, float* mean,
                              float* rstd, int B, int H, int W, int C, void* stream);
 int esvit_patch_merge_ln_bwd(const void* dy, const float* x, const float* mean, const float* rstd,
@@ -51,7 +56,8 @@ int esvit_token_mean_bwd(const float* dpooled, const float* dregion_in, float* d
                          void* stream);
 
 /* ---- PatchEmbed: 4x4/4 conv (3->E) + LayerNorm -------------------------------- models/swin_transformer.py:537-547
- * img fp32 [B,3,H,W]; w fp32 [E,3,4,4]; out fp32 [B,(H/4)*(W/4),E].  bwd ACCUMULATES dw/dbias/dgamma/dbeta. */
+ * img fp32 [B,3,H,W], H and W multiples of 4; w fp32 [E,3,4,4]; out fp32 [B,(H/4)*(W/4),E]; E <= 128 or E = 192.
+ * bwd ACCUMULATES dw/dbias/dgamma/dbeta. */
 int esvit_patch_embed_fwd(const float* img, const float* w, const float* bias, const float* gamma, const float* beta,
                           float eps, float* out, float* mean, float* rstd, int B, int H, int W, int E, void* stream);
 int esvit_patch_embed_bwd(const float* img, const float* w, const float* bias, const float* gamma, const float* mean,
