@@ -4,6 +4,7 @@
     python bench_eval.py knn     # knn_classifier on synthetic ImageNet-shaped features, k in {10, 20, 100, 200}
     python bench_eval.py attn    # forward_selfattention(x, n=2), Swin-T W7, 224^2, B = 1 and 64 (analyze_models.py)
     python bench_eval.py transforms  # the eval_linear.py / eval_knn.py input transforms on the device, B = 128 and 256
+    python bench_eval.py linear  # eval_linear.py's training step (LinearProbeStep), Swin-T W7, n = 4, B = 128, C = 1000
 
 probe: images/s of the CUDA path against the unmodified reference modules (oracle/_ref/, fp32, what eval_linear.py runs)
 on the same GPU and the same seeded weights, with the rel-L2 difference of their outputs.
@@ -25,6 +26,11 @@ collated batches, host -> device copy of the sources included, on bench_augment.
 800x600 and 1600x1200 sources; the worker-side cost per image (JPEG decode + convert('RGB'), record, collate; one
 thread); the unmodified reference transforms' images/s per CPU core on the decoded images (oracle/_ref/, when build()
 installed it); and the Swin-T probe rate (as in `probe`) with the CPU cores the reference transforms need to feed it.
+
+linear: images/s of the linear-probe training step from pinned collated batches (EvalAugment, n = 4 features, the
+step), as a CUDA graph and eager; the same features with the reference's torch classifier loop (per-step synchronize and
+loss.item()); the unmodified reference modules in fp32 with that loop (oracle/_ref/); validation images/s (evaluate);
+and the classifier kernels' time per step (CUDA events around each entry point).
 
 Writes nothing in the tree; card name, power limit and SM clocks are read in the same run.
 """
@@ -294,9 +300,126 @@ def transforms(args) -> dict:
     return res
 
 
+def linear(args) -> dict:
+    """eval_linear.py's training step on Swin-T W7 (n = 4, D = 2304) from pinned collated batches (LinearTrainParams ->
+    EvalAugment -> features -> step): LinearProbeStep as a CUDA graph and eager; the same features with the reference's
+    torch classifier loop (nn.Linear fp32, CrossEntropyLoss, torch.optim.SGD, synchronize + loss.item() per step); the
+    unmodified reference modules in fp32 (oracle/_ref/) with that loop; validation images/s (CenterCropParams, evaluate);
+    and the classifier kernels' time per step from CUDA events around each entry point."""
+    from bench_augment import sources
+    from esvit_b200 import _lib
+    from esvit_b200 import augment as AG
+    from esvit_b200 import probe as PB
+    from esvit_b200.swin_transformer import SwinTransformer
+    from oracle import golden as GD
+    from oracle import reference_import as R
+    from oracle import swin as S
+    spec = dict(S.SWIN_T_W7)
+    depths = list(spec["depths"])
+    m = SwinTransformer(img_size=224, num_classes=0, drop_path_rate=0.0, norm_layer=partial(nn.LayerNorm, eps=1e-6), **spec)
+    sd = GD.seeded_state_dict(GD.recipe(m.state_dict()), 0)
+    m.load_state_dict(sd)
+    m = m.cuda().eval()
+    B, C, D = args.batch, args.classes, 2304
+    lr = 0.001 * B / 256  # eval_linear.py's default lr and its linear scaling rule
+    images = sources(64)
+    aug = AG.EvalAugment()
+    torch.manual_seed(args.seed)
+    g = torch.Generator().manual_seed(args.seed)
+
+    def collated(sampler):
+        out = []
+        for k in range(4):
+            imgs = [images[(k * B + i) % len(images)] for i in range(B)]
+            mb, _ = AG.collate_multicrop([(sampler(torch.from_numpy(im)), 0) for im in imgs], pin_memory=True)
+            out.append((mb, torch.randint(0, C, (B,), generator=g)))
+        return out
+    train, val = collated(AG.LinearTrainParams()), collated(AG.CenterCropParams())
+    res = {"mode": "linear", "arch": "swin_tiny_w7", "batch": B, "n": 4, "dim": D, "classes": C}
+
+    def probe_arm(graph: bool):
+        torch.manual_seed(0)
+        clf = PB.LinearClassifier(D, C).cuda()
+        opt = PB.ProbeSGD(clf.parameters(), lr, momentum=0.9, weight_decay=0)
+        step = PB.LinearProbeStep(m, clf, opt, 4, False, depths, use_cuda_graph=graph, augment=aug)
+        k = [0]
+
+        def run():
+            mb, t = train[k[0] % 4]
+            step(mb, t)
+            k[0] += 1
+        s = _time(run, args.steps, max(args.warmup, 5))  # the graph is captured at the fourth call
+        return s, clf, step
+
+    s_graph, clf, _ = probe_arm(True)
+    s_eager, _, step = probe_arm(False)
+    res["esvit_b200_graph"] = {"s_per_step": s_graph, "images_per_s": B / s_graph}
+    res["esvit_b200_eager"] = {"s_per_step": s_eager, "images_per_s": B / s_eager}
+    names = ["esvit_knn_prep", "esvit_gemm_f32", "esvit_probe_ce", "esvit_gemm_wgrad", "esvit_colsum",
+             "esvit_grad_sumsq_multi", "esvit_sgd_ema_multi"]
+    _lib.time_entry_point(names)
+    _lib.reset_counters()
+    for i in range(args.steps):
+        step(*train[i % 4])
+    torch.cuda.synchronize()
+    per = {}
+    for r in _lib.timed_results():
+        per[r["name"]] = per.get(r["name"], 0.0) + r["ms"] / args.steps
+    _lib.time_entry_point(None)
+    res["classifier_kernels_ms_per_step"] = {k: round(v, 4) for k, v in per.items()}
+    res["classifier_kernels_ms_total"] = round(sum(per.values()), 4)
+
+    def torch_loop(backbone, to_features):
+        torch.manual_seed(0)
+        lin = nn.Linear(D, C).cuda()
+        lin.weight.data.normal_(mean=0.0, std=0.01)
+        lin.bias.data.zero_()
+        opt = torch.optim.SGD(lin.parameters(), lr, momentum=0.9, weight_decay=0)
+        k = [0]
+
+        def run():
+            mb, t = train[k[0] % 4]
+            k[0] += 1
+            x = aug(mb)
+            target = t.cuda(non_blocking=True)
+            with torch.no_grad():
+                f = to_features(backbone, x)
+            loss = nn.CrossEntropyLoss()(lin(f), target)
+            opt.zero_grad()
+            loss.backward()
+            opt.step()
+            torch.cuda.synchronize()
+            loss.item()
+        return _time(run, args.steps, args.warmup)
+
+    s_torch = torch_loop(m, lambda b, x: b.forward_return_n_last_blocks(x, 4, False, depths))
+    res["esvit_b200_features_torch_classifier"] = {"s_per_step": s_torch, "images_per_s": B / s_torch}
+    if R.available():
+        ns = R.load()
+        ref = ns.SwinTransformer(img_size=224, in_chans=3, num_classes=0, embed_dim=spec["embed_dim"], depths=depths,
+                                 num_heads=list(spec["num_heads"]), window_size=spec["window_size"], drop_path_rate=0.0,
+                                 norm_layer=partial(nn.LayerNorm, eps=1e-6))
+        ref.load_state_dict(sd)
+        ref = ref.cuda().eval()
+        s_ref = torch_loop(ref, lambda b, x: b.forward_return_n_last_blocks(x, 4, False, depths))
+        res["reference_fp32"] = {"s_per_step": s_ref, "images_per_s": B / s_ref}
+        res["speedup_graph_vs_reference"] = s_ref / s_graph
+    else:
+        res["reference_fp32"] = "oracle/_ref not installed"
+    PB.evaluate(val[:1], m, clf, 4, False, depths, augment=aug)
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    reps = max(1, args.steps // 4)
+    for _ in range(reps):
+        PB.evaluate(val, m, clf, 4, False, depths, augment=aug)  # ends in its one host synchronisation
+    s_val = (time.perf_counter() - t0) / (reps * len(val))
+    res["validation"] = {"s_per_batch": s_val, "images_per_s": B / s_val}
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("mode", choices=["probe", "knn", "attn", "transforms"])
+    ap.add_argument("mode", choices=["probe", "knn", "attn", "transforms", "linear"])
     ap.add_argument("--batch", type=int, default=128)
     ap.add_argument("--batches", default="1,64", help="attn: batch sizes")
     ap.add_argument("--steps", type=int, default=10)
@@ -316,7 +439,7 @@ def main():
         sys.exit("bench_eval.py needs a CUDA device")
     torch.backends.cuda.matmul.allow_tf32 = False  # the reference arms run fp32
     before = card()
-    res = {"probe": probe, "knn": knn, "attn": attn, "transforms": transforms}[args.mode](args)
+    res = {"probe": probe, "knn": knn, "attn": attn, "transforms": transforms, "linear": linear}[args.mode](args)
     res["card"] = before
     res["card_after"] = card()
     print(json.dumps(res))

@@ -33,6 +33,7 @@ SIGNATURES = {
     "esvit_window_attn_probs": [P, P, P, P, I, P, I, I, I, I, I, I, I, F, P],
     "esvit_gemm_bf16": [P, P, P, P, P, L, I, I, I, I, I, I, P],
     "esvit_gemm_mul_colsum2": [P, P, P, P, P, P, L, I, I, I, I, P],
+    "esvit_gemm_f32": [P, P, P, P, L, I, I, I, P],
     "esvit_gemm_wgrad_ws_floats": [I, I],
     "esvit_gemm_wgrad": [P, P, P, P, L, I, I, I, I, P],
     "esvit_mlp_fwd": [P, P, P, P, P, P, P, P, L, I, P],
@@ -93,6 +94,7 @@ SIGNATURES = {
     "esvit_knn_prep": [P, P, P, P, L, L, I, P],
     "esvit_knn_select": [P, L, P, P, P, P, P, I, I, I, I, I, P, P, P, P, P, P],
     "esvit_knn_vote": [P, P, P, P, L, I, F, I, P, P],
+    "esvit_probe_ce": [P, I, P, I, I, P, P, P, P, P, P, P],
     "esvit_augment_coeffs": [P, P, P, I, I, P],
     "esvit_augment_resize_h": [P, P, P, P, P, I, L, P],
     "esvit_augment_color": [P, P, P, P, P, I, I, I, P],
@@ -149,6 +151,7 @@ def call(name: str, *args) -> None:
 # kernels launched per call of each entry point (entries that launch more than one kernel are computed per call)
 _LAUNCHES = {"esvit_colsum": 2, "esvit_gemm_mul_colsum2": 2, "esvit_gemm_wgrad": 2,
              "esvit_mixup_q": 2,  # GEMM + fold; mixup weights + product
+             "esvit_probe_ce": 2,
              "esvit_headbn_fwd_stats": 2, "esvit_headbn_fwd_apply": 2, "esvit_headbn_bwd_stats": 2,
              "esvit_headbn_bwd_apply": 3}
 _launch_count = 0

@@ -446,18 +446,20 @@ __global__ void __launch_bounds__(384, 1) gemm_kernel(const __grid_constant__ CU
       if (prev >= 0) mbar_arrive(&empty[prev]);
 
       if constexpr (EPI == EPI_F32) {
-        // ---- fp32 split-K partials straight from the registers ----
+        // ---- fp32 split-K partials straight from the registers (+ bias: the unsplit esvit_gemm_f32 only) ----
 #pragma unroll
         for (int i = 0; i < BN / 8; i++) {
           const int col = n0 + i * 8 + frag_col;
           if (col >= p.N) continue;  // N % 8 == 0: col + 1 < N as well, and the test is uniform over the warp
+          const float2 bb = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : make_float2(0.f, 0.f);
 #pragma unroll
           for (int h = 0; h < 2; h++) {
             const int row = m0 + frag_row + 8 * h;
             if (row >= p.M) continue;
             const long long off = (long long)row * p.N + col;
-            *reinterpret_cast<float2*>(p.part + (long long)split * p.M * p.N + off) =
-                make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+            float2 v = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+            if (p.bias) { v.x += bb.x; v.y += bb.y; }   // no bias: the partials as accumulated, signed zeros included
+            *reinterpret_cast<float2*>(p.part + (long long)split * p.M * p.N + off) = v;
           }
         }
         continue;
@@ -950,8 +952,9 @@ static int launch_cfg(const Call& c, void* stream, int* rows_out) {
 
 template <int WG, int BN, int EPI>
 static int launch_majors(const Call& c, void* stream, int* rows_out) {
-  if constexpr (EPI == EPI_F32) {  // weight gradient: both operands MN-major
+  if constexpr (EPI == EPI_F32) {  // weight gradient: both operands MN-major; fp32 forward (esvit_gemm_f32): both K-major
     if (c.a_mn && c.b_mn) return launch_cfg<WG, BN, EPI, 1, 1>(c, stream, rows_out);
+    if (!c.a_mn && !c.b_mn) return launch_cfg<WG, BN, EPI, 0, 0>(c, stream, rows_out);
   } else if constexpr (EPI == EPI_MUL) {
     if (!c.a_mn) return c.b_mn ? launch_cfg<WG, BN, EPI, 0, 1>(c, stream, rows_out) : launch_cfg<WG, BN, EPI, 0, 0>(c, stream, rows_out);
   } else {
@@ -1064,6 +1067,24 @@ ESVIT_API int esvit_gemm_mul_colsum2(const void* a, const void* b, const void* m
   if (rc != 0) return rc;
   hg::colsum_fold_kernel<<<(N + 255) / 256, 256, 0, (cudaStream_t)stream>>>(ws, rows, N, colsum);
   ESVIT_LAUNCH_CHECK();
+}
+
+// out[M,N] (fp32) = a[M,K] . b[N,K]^T + bias[N]: a Linear forward with fp32 output (the linear probe's logits, whose
+// top-5 order bf16 could not resolve).  The fp32 epilogue of the weight gradient with one K split, so every output is
+// one tile's accumulator (+ bias) written once: bit-reproducible.  N, K multiples of 8; bias fp32 [N] or NULL; out
+// 8-byte aligned.  tile as esvit_gemm_bf16.
+ESVIT_API int esvit_gemm_f32(const void* a, const void* b, const float* bias, float* out, long long M, int N, int K,
+                             int tile, void* stream) {
+  if (M <= 0 || N <= 0 || K <= 0 || (N % 8) || (K % 8) || M > 0x7fffffffLL || !out || ((uintptr_t)out & 7) ||
+      ((uintptr_t)bias & 7))
+    return ESVIT_ERR_BAD_ARG;
+  hg::Call c;
+  c.a = a; c.b = b; c.a_mn = 0; c.b_mn = 0;
+  c.p.bias = bias; c.p.out = nullptr; c.p.aux = nullptr; c.p.colsum = nullptr; c.p.part = out;
+  c.p.M = (int)M; c.p.N = N; c.p.K = K; c.p.splits = 1; c.p.kb_per_split = (K + hg::BK - 1) / hg::BK;
+  int wg, bn;
+  hg::pick_tile(M, N, K, tile, false, &wg, &bn);
+  return hg::launch(c, hg::EPI_F32, wg, bn, stream);
 }
 
 // Weight gradient of a Linear: dw[N,K] (fp32) (+)= dy[T,N]^T . x[T,K]   (dy, x bf16 row-major, read as they lie through

@@ -17,12 +17,17 @@ BF16 = torch.bfloat16
 _registry: Dict[int, Tuple[weakref.ref, torch.Tensor, int]] = {}
 
 
-def register(param: torch.Tensor) -> torch.Tensor:
-    """Create (or return) the bf16 shadow of `param`."""
+def register(param: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Create (or return) the bf16 shadow of `param`.  out: bf16 storage for a new shadow, shaped like `param` (e.g. the
+    leading rows of a zero-padded buffer a GEMM reads whole)."""
     ent = _registry.get(id(param))
     if ent is not None and ent[0]() is param:
         return ent[1]
-    shadow = param.detach().to(BF16)
+    if out is None:
+        shadow = param.detach().to(BF16)
+    else:
+        assert out.dtype == BF16 and out.shape == param.shape and out.is_contiguous()
+        shadow = out.copy_(param.detach())
     _registry[id(param)] = (weakref.ref(param), shadow, param._version)
     return shadow
 

@@ -108,6 +108,10 @@ int esvit_gemm_bf16(const void* a, const void* b, const float* bias, void* out, 
                     int a_mn, int b_mn, int act, int tile, void* stream);
 int esvit_gemm_mul_colsum2(const void* a, const void* b, const void* mult, void* out, float* colsum, float* ws,
                            long long M, int N, int K, int b_mn, int tile, void* stream);
+/* gemm_f32: out[M,N] (fp32) = a[M,K] . b[N,K]^T + bias[N] (bias fp32 or NULL), both operands K-major: the fp32 epilogue
+ *   of gemm_wgrad with one K split.  N, K multiples of 8; out 8-byte aligned.  The linear probe's logits. */
+int esvit_gemm_f32(const void* a, const void* b, const float* bias, float* out, long long M, int N, int K, int tile,
+                   void* stream);
 int esvit_gemm_wgrad_ws_floats(int N, int K);
 int esvit_gemm_wgrad(const void* dy, const void* x, float* dw, float* ws, long long T, int N, int K, int accumulate,
                      int tile, void* stream);
@@ -356,6 +360,16 @@ int esvit_knn_select(const void* S, long long ld, const float* a, const float* b
                      float* cand_val, int* count, float* sims, long long* idx, void* stream);
 int esvit_knn_vote(const float* sims, const long long* idx, const long long* train_labels, const long long* test_labels,
                    long long M, int k, float T, int num_classes, long long* hits, void* stream);
+
+/* ---- linear-probe cross-entropy (csrc/probe.cu) ------------------------ eval_linear.py:244-304, utils.py:468-475
+ * probe_ce: per row of logits fp32 [B, ld] (classes [0, C) used; ld % 8 == 0, C <= 12288) with label int64 in [0, C)
+ *   or -1 (padding row): loss = lse - logit[label]; rank of the label by (value desc, index asc); dlogits bf16 [B, ld]
+ *   (or NULL) = (softmax - onehot) / B_valid, zero on padding rows and classes >= C, B_valid = rows with a label >= 0.
+ *   row_loss fp32 [B] and row_rank int32 [B] are scratch.  loss_out fp32 [1] = the batch's mean loss (fixed-order
+ *   fp64 sum); acc fp64 [1] and counts int64 [4] (or both NULL) ACCUMULATE the mean loss and {batches, images, top-1
+ *   hits, top-5 hits}.  No floating-point atomics. */
+int esvit_probe_ce(const float* logits, int ld, const long long* labels, int B, int C, void* dlogits, float* row_loss,
+                   int* row_rank, float* loss_out, double* acc, long long* counts, void* stream);
 
 /* ---- multi-crop augmentation (DataAugmentationDINO) on decoded uint8 images ---------------- datasets/build.py:203-261
  * Pillow's arithmetic for RandomResizedCrop(bicubic) / hflip / ColorJitter / RandomGrayscale / ImageFilter.GaussianBlur /
